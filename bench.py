@@ -1,7 +1,7 @@
 #!/usr/bin/env python3
 """Benchmark of the hot path: fused EKF predict+update steps/s over a batch of independent filters.
 
-  python bench.py --gpus N --steps K --warmup W            # this engine on N B200s (torchrun for N > 1)
+  python bench.py --gpus N --steps K --warmup W            # this engine on N H100s (torchrun for N > 1)
   python bench.py --impl reference --gpus N --steps K ...  # the reference's C path on the host cores
 
 One "step" = one launch of <name>_batch_step_<kind> over the whole per-GPU batch: for every filter
@@ -14,7 +14,7 @@ one predict(dt) + one update_<kind> (rednose/templates/ekf_c.c:8-33 + :37-121). 
 
 Prints ONE JSON line (rank 0).  `value` is the device-resident throughput; `e2e` goes through the public
 BatchedEKF.predict_and_update_batch call with observations in pinned HOST memory and the state estimate
-copied back every step; `roofline` is the dominant kernel against the measured HBM peak; `cpu_baseline`
+copied back every step; `roofline` is the dominant kernel against the HBM peak (MEASURED_PEAKS.json, else the data sheet); `cpu_baseline`
 is the oracle's reference-equivalent C path on the host cores (bounded sample).
 """
 import argparse
@@ -40,7 +40,7 @@ WORKLOADS = {
   "msckf_10k": dict(filter="msckf", batch=10_000, steps=100, warmup=5),         # config 5: triangulation + gated feature update + augment
 }
 LIVE_R = {4: [0.025**2] * 3, 10: [0.5**2] * 3, 12: [5.0**2] * 3}
-L2_BYTES = 126 << 20
+L2_BYTES = 50 << 20
 
 
 def bytes_per_step(dim, edim, m, ea=0):
@@ -53,7 +53,25 @@ def measured_peaks():
     with open(os.path.join(REPO, "MEASURED_PEAKS.json"), encoding="utf-8") as f:
       return float(json.load(f)["hbm_gbs"]), "measured"
   except Exception:  # pylint: disable=broad-except
-    return 6650.0, "fallback"
+    return 3350.0, "H100 SXM data sheet, not measured"
+
+
+DUMP_FILTERS, DUMP_BYTES = 8192, 48 << 20   # --dump-outputs: at most 8192 sampled filters and 48 MB of float64
+
+
+def dump_sample(B, doubles_per_filter):
+  """Sorted indices of a fixed, seeded sample of filters out of B (the same for every build and run), as many as fit
+  DUMP_BYTES at `doubles_per_filter` float64 values each."""
+  n = min(B, DUMP_FILTERS, DUMP_BYTES // (8 * doubles_per_filter))
+  return np.sort(np.random.default_rng(2024).choice(B, n, replace=False))
+
+
+def dump_outputs(out_dir, arrays):
+  """Write each array as <out_dir>/<name>.npy in float64."""
+  os.makedirs(out_dir, exist_ok=True)
+  for name, a in arrays.items():
+    a = a.detach().cpu().numpy() if hasattr(a, "detach") else np.asarray(a)
+    np.save(os.path.join(out_dir, f"{name}.npy"), np.ascontiguousarray(a, dtype=np.float64))
 
 
 def kind_schedule(filter_name, n):
@@ -63,7 +81,7 @@ def kind_schedule(filter_name, n):
 
 
 class ClockSampler:
-  """nvidia-smi clocks / throttle reasons DURING the timed region (B200_PROFILING.md recipe)."""
+  """nvidia-smi clocks / throttle reasons DURING the timed region."""
   Q = "clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap"
 
   def __init__(self, gpu_index):
@@ -221,6 +239,10 @@ def run_gpu(args):
   for j in range(args.steps):
     per_kind.setdefault(sched[args.warmup + j], []).append(ev[j][0].elapsed_time(ev[j][1]))
   assert bool(torch.isfinite(eng.x).all()), "filter diverged during the benchmark"
+  if args.dump_outputs and rank == 0:
+    # what the last timed step returned to its caller: the state estimate, its covariance and the innovation y
+    sel = torch.as_tensor(dump_sample(B, dim + edim * edim + max(zdim.values()) + 1), device=dev)
+    dump_outputs(args.dump_outputs, {"x": eng.x[sel], "P": eng.P[sel], "y": zwork[sched[args.warmup + args.steps - 1]][sel, 0], "filter_index": sel})
 
   # ---- sustained figure: the same loop for >= args.sustain seconds (power-capped clocks, not a burst) ----
   sustained = None
@@ -444,7 +466,7 @@ def run_gpu(args):
       "dtype": "f64", "data": "synthetic",
       "config": {"workload": args.workload, "filter": fname, "filters_per_gpu": B, "dim": dim, "edim": edim,
                  "kind_schedule": "live: kinds 4/10 alternating + kind 12 every 100 steps" if fname == "live" else "kind 1",
-                 "l2": f"inputs larger than L2 ({8 * B * edim * edim / 2**20:.0f} MiB of P per GPU vs 126 MiB)" if 8 * B * edim * edim > L2_BYTES else "inputs FIT in L2 (126 MiB)",
+                 "l2": f"inputs larger than L2 ({8 * B * edim * edim / 2**20:.0f} MiB of P per GPU vs 50 MiB)" if 8 * B * edim * edim > L2_BYTES else "inputs FIT in L2 (50 MiB)",
                  "sharding": "independent filters per GPU, no data-path collective"},
       "gpu_launches": launches,
       "per_kind_ms": {str(k): float(np.mean(v)) for k, v in per_kind.items()},
@@ -588,6 +610,7 @@ def run_rts(args):
   ev_ready = [torch.cuda.Event() for _ in range(2)]
   ev_done = [torch.cuda.Event() for _ in range(2)]
   chk = {"finite": True, "n": 0, "k": 0}
+  dump_sel, dumped = torch.as_tensor(dump_sample(B, dim + edim * edim + 1), device=dev), {}
 
   def sink(lo, hi, k0, xs, Ps):
     n = xs.shape[0]
@@ -606,6 +629,9 @@ def run_rts(args):
     chk["n"] += n * (hi - lo)
     if k0 == 0:
       chk["finite"] = chk["finite"] and bool(torch.isfinite(xs[0]).all()) and bool(torch.isfinite(Ps[0]).all())
+      if args.dump_outputs:   # smoothed estimate of the first history step; the last pass overwrites the earlier ones
+        rows = dump_sel[(dump_sel >= lo) & (dump_sel < hi)] - lo
+        dumped[lo] = (xs[0, rows].clone(), Ps[0, rows].clone())
 
   def sync_all():
     torch.cuda.synchronize(dev)
@@ -636,6 +662,9 @@ def run_rts(args):
   elapsed_ms, fwd_ms, refwd_ms, bwd_ms = _max_over_ranks(torch, dist, world, dev, [t0.elapsed_time(t1), acc["forward_ms"], acc["reforward_with_history_ms"], acc["backward_ms"]])
   launches = cs._engine.launches - launches0
   assert chk["finite"] and chk["n"] == B * T * args.steps, (chk, B * T * args.steps)
+  if args.dump_outputs and rank == 0:
+    dump_outputs(args.dump_outputs, {"x_smoothed_step0": torch.cat([dumped[lo][0] for lo in sorted(dumped)]),
+                                     "P_smoothed_step0": torch.cat([dumped[lo][1] for lo in sorted(dumped)]), "filter_index": dump_sel})
   if rank == 0:
     peak, peak_kind = measured_peaks()
     K = args.steps
@@ -660,8 +689,8 @@ def run_rts(args):
                  "other_ms": elapsed_ms - fwd_ms - refwd_ms - bwd_ms,
                  "reforward_frac_of_peak": (8240 + 8120) * refwd_steps / (refwd_ms * 1e-3) / 1e9 / peak, "forward_frac_of_peak": 8240 * B * T * K / (fwd_ms * 1e-3) / 1e9 / peak},
       "roofline": {"bound": "hbm", "kernel": "ekf_rts_warp_mma<live>", "achieved": ach, "peak": peak, "unit": "GB/s", "frac": ach / peak, "peak_source": peak_kind,
-                   "algorithmic_bytes_per_step": 12176, "traffic": None, "traffic_source": "see profiles/ (ncu capture of the backward kernel)",
-                   "note": "the backward step is ~45k FP64 FMA per filter-step (LDL^T, two triangular solves, two 24^3 products): at 64 FMA/clk/SM that alone is ~0.7 of this HBM roofline, so the kernel is FP64-pipe/latency bound, not bandwidth bound (DESIGN.md)"},
+                   "algorithmic_bytes_per_step": 12176, "traffic": None, "traffic_source": "not measured",
+                   "note": "the backward step is ~45k FP64 FMA per filter-step (LDL^T, two triangular solves, two 24^3 products): at 64 FMA/clk/SM on 132 SMs at 1.98 GHz that alone takes ~0.85 of the time of this HBM roofline, so the kernel is FP64-pipe/latency bound as much as bandwidth bound (DESIGN.md)"},
       "e2e": {"value": B * T * K * world / (elapsed_ms * 1e-3), "unit": "steps/s", "h2d_bytes_per_step": counters["h2d"] / K, "d2h_bytes_per_step": counters["d2h"] / K,
               "what": "the timed region IS end to end: every step's observations are copied from pinned host memory (twice: both forward passes) and the smoothed pose columns of every step go back to pinned host memory"},
       "clocks": clocks.summary(), "numa_node": numa,
@@ -799,10 +828,13 @@ def run_msckf(args):
     for j in range(K):
       z, outl = make_obs()                                  # synthetic camera frame: NOT part of the timed hot path
       ev[j][0].record()
-      hot_path(z)
+      pos_last = hot_path(z)
       ev[j][1].record()
       stats["tracks"] += B
     sync_all()
+  if args.dump_outputs and rank == 0:
+    sel = torch.as_tensor(dump_sample(B, DIM + EDIM * EDIM + 3 + 1), device=dev)
+    dump_outputs(args.dump_outputs, {"x": eng.x[sel], "P": eng.P[sel], "point": pos_last[sel], "filter_index": sel})
   hot_ms = sum(a.elapsed_time(b) for a, b in ev)
   (hot_ms,) = _max_over_ranks(torch, dist, world, dev, [hot_ms])
   launches = 2 * (eng.launches - launches0) + K   # leaf + CTA kernel per fused step (the augment rides in the CTA kernel), + compute_pos per frame
@@ -846,13 +878,13 @@ def run_msckf(args):
       "config": {"workload": "msckf_10k", "filter": "msckf", "filters_per_gpu": B, "dim": DIM, "edim": EDIM, "clones": 10, "zdim": 20, "projected_dim": 17,
                  "outlier_fraction": 0.05, "gated_fraction_measured": float(gated.double().mean()), "outliers_among_gated": float((outl & gated).sum() / max(1, int(gated.sum()))),
                  "gauss_newton_iterations_mean": float(iters.abs().double().mean()), "triangulations_failed_fraction": float((~ok).double().mean()),
-                 "l2": f"state {B * EDIM * EDIM * 8 / 2**20:.0f} MiB of P vs 126 MiB of L2: {'larger than L2' if B * EDIM * EDIM * 8 > L2_BYTES else 'FITS in L2'}",
+                 "l2": f"state {B * EDIM * EDIM * 8 / 2**20:.0f} MiB of P vs 50 MiB of L2: {'larger than L2' if B * EDIM * EDIM * 8 > L2_BYTES else 'FITS in L2'}",
                  "timing": "CUDA events around the hot-path calls of every frame; the synthetic observation generator between frames is excluded",
                  "sharding": "independent filters per GPU, no data-path collective"},
       "gpu_launches": launches,
       "roofline": {"bound": "hbm", "kernel": "ekf_step_cta<msckf, kind 17> (+ leaf, compute_pos, augment in the same timed region)", "achieved": bs * B / (step_ms * 1e-3) / 1e9, "peak": peak, "unit": "GB/s",
                    "frac": bs * B / (step_ms * 1e-3) / 1e9 / peak, "peak_source": peak_kind, "algorithmic_bytes_per_step": bs, "traffic": None,
-                   "traffic_source": "see profiles/ (ncu capture of ekf_step_cta)"},
+                   "traffic_source": "not measured"},
       "e2e": {"value": B * e2e_K * world / (e2e_ms * 1e-3), "unit": "steps/s", "h2d_bytes_per_step": B * 20 * 8, "d2h_bytes_per_step": B * DIM * 8, "steps": e2e_K,
               "what": "per frame: z [B, 20] from pinned host memory, compute_pos + fused step + augment, x [B, 93] back to pinned host memory; P stays resident"},
       "clocks": clocks.summary(), "numa_node": numa,
@@ -1098,9 +1130,8 @@ class CpuArm:
 
 
 def _cpu_limits():
-  """(logical CPUs this process may run on, cgroup CPU quota in CPUs or None).  The GPU boxes of this pool run the
-  container under a CFS quota (cpu.max) far below the 128 logical CPUs the affinity mask shows; threads beyond the quota
-  are throttled, not run (measured: linear to the quota, then flat, then worse -- profiles/r02_cpu_thread_sweep.txt)."""
+  """(logical CPUs this process may run on, cgroup CPU quota in CPUs or None).  A container may run under a CFS quota
+  (cpu.max) far below the logical CPUs the affinity mask shows; threads beyond the quota are throttled, not run."""
   try:
     n = len(os.sched_getaffinity(0))
   except AttributeError:
@@ -1305,8 +1336,10 @@ def main():
   ap.add_argument("--sustain", type=float, default=2.0, help="seconds of the sustained figure beside the K-step burst (0 = skip)")
   ap.add_argument("--rts-steps", type=int, default=1000, help="live_rts: history length T (BASELINE.json: 10000)")
   ap.add_argument("--rts-segment", type=int, default=50, help="live_rts: steps between checkpoints")
-  ap.add_argument("--hbm-budget-gb", type=float, default=140.0, help="live_rts: HBM the smoother may use per GPU")
+  ap.add_argument("--hbm-budget-gb", type=float, default=60.0, help="live_rts: HBM the smoother may use per GPU")
   ap.add_argument("--no-cpu-baseline", action="store_true")
+  ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                  help="after the timed steps, write what the last one computed (a fixed sample of filters) as DIR/<name>.npy")
   ap.add_argument("--no-extras", dest="extras", action="store_false",
                   help="skip the short measurements of the other kernels (kinematic / history / RTS / ragged / MSCKF, ~1 min)")
   ap.add_argument("--extras", dest="extras", action="store_true", default=True)

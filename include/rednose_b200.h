@@ -1,4 +1,4 @@
-/* rednose_b200 -- C-ABI of the B200-native batched EKF engine.
+/* rednose_b200 -- C-ABI of the H100-native batched EKF engine.
  *
  * This header declares (1) the plugin descriptor every generated lib<name>.so returns
  * from ekf_get(), the plain-C replacement of the reference's C++ `struct EKF` +

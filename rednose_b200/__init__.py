@@ -1,4 +1,4 @@
-"""rednose_b200 -- B200-native batched EKF engine behind commaai/rednose's filter-definition surface.
+"""rednose_b200 -- H100-native batched EKF engine behind commaai/rednose's filter-definition surface.
 
 Public entry points (see DESIGN.md / INTEGRATION.md):
 

@@ -1,4 +1,4 @@
-"""Batched EKF engine: B independent filter instances resident in B200 HBM.
+"""Batched EKF engine: B independent filter instances resident in H100 HBM.
 
 This is the batched counterpart of the reference's per-instance driver
 (rednose/helpers/ekf_sym.cc:158-219 / ekf_sym.py:484-531): the state ``x[B, DIM]`` and

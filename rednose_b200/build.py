@@ -2,7 +2,7 @@
 
 Stands in for the reference's SCons tool (site_scons/site_tools/rednose_filter.py:27-37:
 run the generator, then link ``lib{target}.so``) with a direct nvcc invocation for
-sm_100a.  Everything is built in-tree so the artefacts travel with the repository.
+sm_90a.  Everything is built in-tree.
 """
 import os
 import shutil
@@ -14,7 +14,7 @@ INCLUDE_DIR = os.path.abspath(os.path.join(PKG_DIR, "..", "include"))
 GENERATED_DIR = os.environ.get("REDNOSE_B200_GENERATED_DIR") or os.path.join(PKG_DIR, "generated")
 
 NVCC_FLAGS = [
-  "-gencode", "arch=compute_100a,code=sm_100a",
+  "-gencode", "arch=compute_90a,code=sm_90a",
   "-O3", "-lineinfo", "-std=c++17", "--expt-relaxed-constexpr",
   "-Xcompiler", "-fPIC", "-shared",
 ]
@@ -55,7 +55,7 @@ def csrc_sources():
 
 
 def compile_filter(folder, name, force=False, verbose=False):
-  """``{folder}/{name}.cu`` -> ``{folder}/lib{name}.so`` (sm_100a)."""
+  """``{folder}/{name}.cu`` -> ``{folder}/lib{name}.so`` (sm_90a)."""
   src = os.path.join(folder, f"{name}.cu")
   lib = os.path.join(folder, f"lib{name}.so")
   if not force and _newer(lib, [src] + csrc_sources()) and _flags_match(folder, name):

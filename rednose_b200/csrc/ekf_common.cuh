@@ -1,4 +1,4 @@
-// rednose_b200 -- common device/host helpers for the batched EKF kernels (sm_100a).
+// rednose_b200 -- common device/host helpers for the batched EKF kernels (sm_90a).
 //
 // Hot path being replaced: rednose/templates/ekf_c.c:8-33 (predict) and :37-121 (update),
 // plus the driver-level quaternion normalisation rednose/helpers/ekf_sym.cc:69-77.

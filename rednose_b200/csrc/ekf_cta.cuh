@@ -231,7 +231,7 @@ __global__ void __launch_bounds__(cta_threads<M>(), RNB_CTA_MIN_BLOCKS) ekf_step
   constexpr int NC = (E + 31) / 32;     // 32-column chunks of a row
   // cp.async (LDGSTS, 8 bytes per element: a packed row starts 16-byte aligned only every other row): no registers are
   // held, so the whole triangle is in flight at once -- ONE global round trip, overlapped with the leaf-value loads below
-  // (the register-staged version needed four and spent 23 % of the kernel waiting on them, profiles/r02_cta_ncu_summary.txt)
+  // (the register-staged version needed four and spent a large share of the kernel waiting on them)
   for (int i = warp; i < E; i += nw) {
     const int ti = i * (i + 1) / 2;
 #pragma unroll

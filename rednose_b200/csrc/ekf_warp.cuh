@@ -11,7 +11,7 @@
 //       H_err = H * H_mod, y = z - h.  Results go to a per-filter ROW in shared memory.  The leaf
 //       code is scalar and branch-free, so 32 lanes = 32 different filters run it at full SIMT
 //       efficiency -- evaluating it redundantly in every lane of a warp-per-filter kernel was the
-//       dominant cost of the first version (profiles/r01_a_*).
+//       dominant cost of the first version.
 //  B  (warp-per-filter)    for each filter of the group in turn: lane j holds COLUMN j of the
 //       symmetric covariance P in registers.  With that ownership
 //         (F P)[:,j] = F P[:,j]            lane-local  (generated sparse MODEL::F_apply)
@@ -282,8 +282,8 @@ __global__ void __launch_bounds__(W * 32, RNB_MIN_WARPS / W) ekf_step_warp(const
 
     // ---- stage this group's small per-filter records into the rows (coalesced) ----
     // every global load of the block (x, z, R, dt) is issued before the first shared-memory store that depends on
-    // one of them: the group pays ONE global round trip here instead of one per record type (profiles/r01_f: four
-    // serialised long-scoreboard waits = 10 % of the kernel's samples)
+    // one of them: the group pays ONE global round trip here instead of one per record type (four serialised
+    // long-scoreboard waits otherwise)
     double dt_lane = a.dt;
     {
       StageRegs<D, G> rx;

@@ -6,8 +6,7 @@
 //   half-warp h (lanes 16h .. 16h+15) works on filter f + h of the group; lane hl of the half owns the ADJACENT
 //   columns 2 hl and 2 hl + 1 of that filter's covariance.
 //
-// Why: ekf_step_warp is bound by the L1TEX data pipe (profiles/r01_f: l1tex__data_pipe_lsu_wavefronts 85 % of
-// peak, 264 shared-memory wavefronts per filter).  160 of those are warp-uniform ("broadcast") loads of per-filter
+// Why: ekf_step_warp is bound by the L1TEX data pipe (shared-memory wavefronts per filter).  Most of those are warp-uniform ("broadcast") loads of per-filter
 // values -- F slots, H slots, the rows of H P for the rank-m update -- and a broadcast costs one wavefront per
 // 8 bytes no matter how many lanes listen.  Here one such instruction fetches the value of filter f for half 0 and
 // of filter f+1 for half 1, and serves two columns per lane: broadcast wavefronts per filter halve.  Adjacent

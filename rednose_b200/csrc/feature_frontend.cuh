@@ -1,4 +1,4 @@
-// rednose_b200 -- MSCKF front-end kernels: batched feature-track triangulation and track bookkeeping (sm_100a).
+// rednose_b200 -- MSCKF front-end kernels: batched feature-track triangulation and track bookkeeping (sm_90a).
 //
 // Replaces, for a batch of independent tracks / camera frames,
 //   rednose/templates/compute_pos.c:10-27   gauss_newton()   (Eigen 2K x 3 least squares, <= 30 iterations)
@@ -135,8 +135,8 @@ __global__ void __launch_bounds__(CP_THREADS) compute_pos_thread(const double* _
 // One LANE per (track, pose): the K pose terms of a Gauss-Newton iteration are independent, so a group of LPT >= K lanes
 // evaluates them at once and butterfly-reduces the 9 sums of the normal equations (every lane of the group ends with
 // bit-identical sums: the xor tree is symmetric and IEEE addition commutes), then every lane solves the same 3 x 3.  The
-// dependent chain of an iteration is one pose term instead of K of them: 86 -> ~15 us for the 10 000 tracks of config 5,
-// where the thread-per-track kernel is pure latency (profiles/r02_compute_pos_ncu_summary.txt).  The sums are formed in
+// dependent chain of an iteration is one pose term instead of K of them, at the 10 000 tracks of config 5
+// where the thread-per-track kernel is pure latency.  The sums are formed in
 // tree order instead of the reference's row order (compute_pos.c:22): same algorithm, last-bit differences.
 template <class FM, int LPT>
 __global__ void __launch_bounds__(128) compute_pos_lanes(const double* __restrict__ to_c, const double* __restrict__ poses, const double* __restrict__ img,

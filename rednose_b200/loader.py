@@ -47,4 +47,4 @@ def raise_on_cuda_error(lib, name, what=""):
     return
   status = status_fn()
   if status != 0:
-    raise RuntimeError(f"rednose_b200: CUDA error {status} in {name} {what} (no CPU fallback exists; a B200 is required)")
+    raise RuntimeError(f"rednose_b200: CUDA error {status} in {name} {what} (no CPU fallback exists; an H100 is required)")

@@ -77,7 +77,7 @@ class RewindingScheduler(RaggedScheduler):
 
   def __init__(self, engine, zdims, depth=16, max_rewind_age=1.0, ea_dims=None, packed=False):
     """packed=True stores the covariance snapshots as their lower triangle (EDIM (EDIM + 1) / 2 doubles instead of EDIM^2:
-    half the ring -- the reference's 512-deep ring then fits 100 000 live filters in one B200's HBM); a restored covariance
+    half the ring -- the reference's 512-deep ring then fits 100 000 live filters in one H100's HBM); a restored covariance
     is then exactly symmetric (upper := lower), which differs from the stored one by the kernels' last-bit asymmetry."""
     super().__init__(engine)
     B, dev = engine.B, engine.device

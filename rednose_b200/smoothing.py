@@ -22,7 +22,7 @@ def history_bytes_per_filter(dim_x, dim_err, T, smoothed_in_place=True):
 
 
 class TiledSmoother:
-  def __init__(self, folder, name, Q, dim_x, dim_err, quaternion_idxs=(), device="cuda", hbm_budget_bytes=120 << 30, tile=None):
+  def __init__(self, folder, name, Q, dim_x, dim_err, quaternion_idxs=(), device="cuda", hbm_budget_bytes=60 << 30, tile=None):
     self.folder, self.name, self.Q = folder, name, Q
     self.dim_x, self.dim_err = dim_x, dim_err
     self.quat = tuple(quaternion_idxs)
@@ -76,7 +76,7 @@ class CheckpointedSmoother:
   """Forward filter + RTS smoother over histories too long to store, for LARGE tiles of filters.
 
   Tiling over filters alone (TiledSmoother) trades history length for batch size: BASELINE.json config 4 (10 000 steps)
-  would leave ~1 500 filters per launch, which cannot fill 148 SMs.  Here only a CHECKPOINT (x, P: 4 kB per live filter)
+  would leave ~1 500 filters per launch, which cannot fill 132 SMs.  Here only a CHECKPOINT (x, P: 4 kB per live filter)
   is kept every `segment` steps of a first forward pass; the backward sweep then visits the segments last to first,
   re-runs the forward filter of one segment from its checkpoint WITH history (segment + 1 steps: the extra one is the
   first step of the segment behind it, whose predicted state the recursion needs) and smooths it starting from the
@@ -85,7 +85,7 @@ class CheckpointedSmoother:
   the price is a second forward pass.  The kernels are deterministic, so the result is bit-identical to smoothing the
   whole history at once (tests/test_parity_gpu.py::test_checkpointed_smoother_equals_full_history)."""
 
-  def __init__(self, folder, name, Q, dim_x, dim_err, quaternion_idxs=(), device="cuda", hbm_budget_bytes=120 << 30, segment=64, tile=None):
+  def __init__(self, folder, name, Q, dim_x, dim_err, quaternion_idxs=(), device="cuda", hbm_budget_bytes=60 << 30, segment=64, tile=None):
     self.folder, self.name, self.Q = folder, name, Q
     self.dim_x, self.dim_err = dim_x, dim_err
     self.quat = tuple(quaternion_idxs)

@@ -1,4 +1,4 @@
-# A/B of the warp-kernel variants on one B200 (run through gpurun): parity tests, bench per variant, one ncu capture
+# A/B of the warp-kernel variants on one H100: parity tests, bench per variant, one ncu capture
 set -x
 python -m pytest tests -m gpu -x -q 2>&1 | tail -4
 run() {  # label, env...

@@ -1,4 +1,4 @@
-# end-of-round validation on one B200 (run through gpurun): parity tests, smoke, default bench, launch list
+# validation on one H100: parity tests, smoke, default bench, launch list
 python -m pytest tests -m gpu -x -q 2>&1 | tail -3
 python -c "import __graft_entry__ as g; g.smoke()" 2>&1 | tail -2
 S=$(date +%s); python bench.py > gpurun_out/bench_final_r1.json 2> gpurun_out/bench_final_r1.err; E=$(date +%s); echo "default bench wall $((E-S)) s"

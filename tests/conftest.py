@@ -9,7 +9,7 @@ if REPO not in sys.path:
 
 
 def pytest_configure(config):
-  config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box)")
+  config.addinivalue_line("markers", "gpu: needs a CUDA device (an H100)")
 
 
 @pytest.fixture(scope="session")
@@ -33,5 +33,5 @@ def oracle_dir():
       build_ref.build(n)
   missing = [n for n in names if not os.path.exists(os.path.join(build_ref.OUT, f"lib{n}.so"))]
   if missing:
-    pytest.skip(f"oracle/_ref not built for {missing} and /root/reference not mounted")
+    pytest.skip(f"oracle/_ref not built for {missing} and the reference checkout is not present")
   return build_ref.OUT

@@ -1,4 +1,4 @@
-"""CPU tests (no GPU): the generated CUDA libraries build for sm_100a, load, and export every
+"""CPU tests (no GPU): the generated CUDA libraries build for sm_90a, load, and export every
 symbol their headers declare; the plugin descriptor is readable.  No compute calls."""
 import ctypes
 import os

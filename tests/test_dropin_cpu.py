@@ -1,8 +1,11 @@
-"""CPU tests of the drop-in surface: the reference's UNMODIFIED example files (read from /root/reference,
-skipped where it is not mounted) import `rednose.helpers.*`, which this repository provides as a shim over
-rednose_b200.  Generation goes through this package's gen_code; running goes through this package's
-EKF_sym_pyx (native driver) -- pointed at the oracle's CPU build of the same C-ABI, since there is no GPU here."""
-import importlib.util
+"""CPU tests of the drop-in surface: filter scripts written against the reference's surface generate and run through this
+package.  The reference's UNMODIFIED example scripts import `rednose.helpers.*`, which this repository provides as a
+shim over rednose_b200; what they generate through it is stored in tests/golden/dropin_reference.json (written by
+tests/golden/make_golden_support.py) and compared here with what this repository's own filter scripts generate.
+Running goes through this package's EKF_sym_pyx (native driver) -- pointed at the oracle's CPU build of the same C-ABI,
+since there is no GPU here."""
+import hashlib
+import json
 import os
 import re
 import runpy
@@ -11,42 +14,45 @@ import sys
 import numpy as np
 import pytest
 
-REF_EXAMPLES = "/root/reference/examples"
-pytestmark = pytest.mark.skipif(not os.path.exists(REF_EXAMPLES), reason="/root/reference not mounted")
+HERE = os.path.dirname(os.path.abspath(__file__))
+FILTERS = os.path.join(os.path.dirname(HERE), "rednose_b200", "filters")
+with open(os.path.join(HERE, "golden", "dropin_reference.json"), encoding="utf-8") as _f:
+  GOLDEN_GEN = json.load(_f)
 
 
-def _load(path, modname):
-  spec = importlib.util.spec_from_file_location(modname, path)
-  mod = importlib.util.module_from_spec(spec)
-  spec.loader.exec_module(mod)
-  return mod
-
-
-def _protos(path):
+def _protos_sha256(path):
   with open(path, encoding="utf-8") as f:
-    return sorted(re.sub(r"\s+", " ", ln) for ln in f.read().split("\n") if ln.startswith("void "))
+    protos = sorted(re.sub(r"\s+", " ", ln) for ln in f.read().split("\n") if ln.startswith("void "))
+  return hashlib.sha256("\n".join(protos).encode()).hexdigest()
+
+
+def _sig(path):
+  with open(path, encoding="utf-8") as f:
+    return re.findall(r"static constexpr int (?:NF|KIND) = [^;]*;", f.read())
 
 
 @pytest.mark.parametrize("script,name", [("kinematic_kf.py", "kinematic"), ("live_kf.py", "live")])
 def test_reference_generator_scripts_run_unchanged(tmp_path, monkeypatch, gen_dir, script, name):
-  """`python <filter>.py <target> <output_dir>` (site_scons/site_tools/rednose_filter.py:13) through this package."""
+  """`python <filter>.py <target> <output_dir>` (site_scons/site_tools/rednose_filter.py:13) through this package
+  generates what the reference's examples/<script> generates through it (stored in GOLDEN_GEN[name])."""
   import rednose
   assert "rednose_b200" in open(os.path.join(os.path.dirname(rednose.__file__), "helpers", "ekf_sym.py")).read()
   monkeypatch.setenv("REDNOSE_B200_NO_COMPILE", "1")
-  monkeypatch.setattr(sys, "argv", [script, name, str(tmp_path)])
-  runpy.run_path(os.path.join(REF_EXAMPLES, script), run_name="__main__")
+  monkeypatch.setattr(sys, "argv", [f"{name}.py", name, str(tmp_path)])
+  runpy.run_path(os.path.join(FILTERS, f"{name}.py"), run_name="__main__")
   assert os.path.exists(tmp_path / f"{name}.cu") and os.path.exists(tmp_path / f"{name}.h")
-  # same C-ABI as the library built from this repository's own definition of the model
-  assert _protos(tmp_path / f"{name}.h") == _protos(os.path.join(gen_dir, f"{name}.h"))
-  # same structure: the sparsity signature of F / H_err survives (33 F slots, per-kind non-zeros)
-  sig = lambda p: re.findall(r"static constexpr int (?:NF|KIND) = [^;]*;", open(p).read())
-  assert sig(tmp_path / f"{name}.cu") == sig(os.path.join(gen_dir, f"{name}.cu"))
+  for d in (str(tmp_path), gen_dir):
+    # same C-ABI as the reference's example script generates
+    assert _protos_sha256(os.path.join(d, f"{name}.h")) == GOLDEN_GEN[name]["protos_sha256"]
+    # same structure: the sparsity signature of F / H_err survives (33 F slots, per-kind non-zeros)
+    assert _sig(os.path.join(d, f"{name}.cu")) == GOLDEN_GEN[name]["sig"]
 
 
 def test_reference_kinematic_example_on_the_dropin_driver(oracle_dir):
-  """examples/test_kinematic_kf.py:10-55 with the reference's own KinematicKalman class."""
+  """examples/test_kinematic_kf.py:10-55 with this package's KinematicKalman (the example's model on the KalmanFilter
+  surface); GOLDEN are the reference test's own expected values."""
+  from rednose_b200.filters import kinematic as mod
   from tests.test_oracle_cpu import GOLDEN
-  mod = _load(os.path.join(REF_EXAMPLES, "kinematic_kf.py"), "ref_kinematic_kf")
   np.random.seed(0)
   kf = mod.KinematicKalman(oracle_dir)
   assert type(kf.filter).__module__ == "rednose_b200.ekf_sym_pyx"
@@ -62,8 +68,9 @@ def test_reference_kinematic_example_on_the_dropin_driver(oracle_dir):
 
 
 def test_reference_live_example_on_the_dropin_driver(oracle_dir):
-  """examples/live_kf.py's LiveKalman: uses .x as a live (DIM,1) view, .filter_time, rts_smooth (live_kf.py:269-306)."""
-  mod = _load(os.path.join(REF_EXAMPLES, "live_kf.py"), "ref_live_kf")
+  """The usage of examples/live_kf.py's LiveKalman (live_kf.py:269-306) on this package's LiveKalman: the quaternion
+  normalisation written through the filter's live (DIM, 1) view, .t, rts_smooth."""
+  from rednose_b200.filters import live as mod
   K = mod.ObservationKind
   kf = mod.LiveKalman(oracle_dir)
   rng = np.random.default_rng(0)
