@@ -163,15 +163,18 @@ inline void launch_step(const StepArgs<M::NG>& a, cudaStream_t st) {
   check(cudaGetLastError(), "ekf_step launch");
 }
 
+// false (and nothing filled) when the quaternion list is invalid: the caller launches nothing
 template <class M>
-inline void fill_common(StepArgs<M::NG>& a, HostCtx<M>& ctx, long long B, const int* quat_idxs, int n_quat, int flags) {
+inline bool fill_common(StepArgs<M::NG>& a, HostCtx<M>& ctx, long long B, const int* quat_idxs, int n_quat, int flags) {
+  if (!check_quat_idxs(quat_idxs, n_quat, M::DIM)) return false;
   memset(&a, 0, sizeof(a));
   a.B = B;
   a.flags = flags;
-  a.n_quat = n_quat < 0 ? 0 : (n_quat > MAX_QUAT ? MAX_QUAT : n_quat);
-  for (int i = 0; i < a.n_quat; ++i) a.quat_idx[i] = quat_idxs[i];
+  a.n_quat = n_quat;
+  for (int i = 0; i < n_quat; ++i) a.quat_idx[i] = quat_idxs[i];
   for (int i = 0; i < (M::NG > 0 ? M::NG : 1); ++i) a.gv[i] = ctx.gv.v[i];
   a.n_obs = 1;
+  return true;
 }
 
 // ----------------------------------------------------------- batched (device) ---
@@ -180,7 +183,7 @@ inline void batch_predict(HostCtx<M>& ctx, double* x, double* P, const double* Q
                           long long B, const int* quat_idxs, int n_quat, int flags,
                           double* hx_pred, double* hP_pred, void* stream) {
   StepArgs<M::NG> a;
-  fill_common<M>(a, ctx, B, quat_idxs, n_quat, flags);
+  if (!fill_common<M>(a, ctx, B, quat_idxs, n_quat, flags)) return;
   a.x = x; a.P = P; a.Q = Q; a.dt_arr = dt_arr; a.dt = dt;
   a.hx_pred = hx_pred; a.hP_pred = hP_pred;
   launch_step<M, NullKind, true, false>(a, (cudaStream_t)stream);
@@ -193,7 +196,7 @@ inline void batch_step(HostCtx<M>& ctx, double* x, double* P, const double* Q, c
                        double* hx_pred, double* hP_pred, double* hx_filt, double* hP_filt, void* stream,
                        const int* idx = nullptr) {
   StepArgs<M::NG> a;
-  fill_common<M>(a, ctx, B, quat_idxs, n_quat, flags);
+  if (!fill_common<M>(a, ctx, B, quat_idxs, n_quat, flags)) return;
   a.idx = idx;
   a.x = x; a.P = P; a.Q = Q; a.dt_arr = dt_arr; a.dt = dt;
   a.z = z; a.R = R; a.ea = (K::EADIM > 0) ? ea : nullptr; a.ea_dim = K::EADIM; a.n_obs = n_obs;
@@ -223,13 +226,14 @@ inline void batch_rts(HostCtx<M>& ctx, const double* hx_pred, const double* hP_p
                       const double* t, int t_per_filter, double* xs, double* Ps, int T, long long B,
                       const int* quat_idxs, int n_quat, int norm_quats, void* stream,
                       const double* x_term = nullptr, const double* P_term = nullptr, long long k0 = 0) {
+  if (!check_quat_idxs(quat_idxs, n_quat, M::DIM)) return;
   RtsArgs<M::NG> a;
   memset(&a, 0, sizeof(a));
   a.x_term = (x_term && P_term) ? x_term : nullptr; a.P_term = (x_term && P_term) ? P_term : nullptr; a.k0 = k0;
   a.hx_pred = hx_pred; a.hP_pred = hP_pred; a.hx_filt = hx_filt; a.hP_filt = hP_filt;
   a.t = t; a.t_per_filter = t_per_filter; a.xs = xs; a.Ps = Ps; a.T = T; a.B = B; a.norm_quats = norm_quats;
-  a.n_quat = n_quat < 0 ? 0 : (n_quat > MAX_QUAT ? MAX_QUAT : n_quat);
-  for (int i = 0; i < a.n_quat; ++i) a.quat_idx[i] = quat_idxs[i];
+  a.n_quat = n_quat;
+  for (int i = 0; i < n_quat; ++i) a.quat_idx[i] = quat_idxs[i];
   for (int i = 0; i < (M::NG > 0 ? M::NG : 1); ++i) a.gv[i] = ctx.gv.v[i];
   launch_rts_auto<M>(a, (cudaStream_t)stream);
 }
@@ -244,6 +248,7 @@ inline void host_step(HostCtx<M>& ctx, double* x, double* P, const double* Q, co
                       double* z, const double* R, const double* ea, int n_obs, long long B,
                       const int* quat_idxs, int n_quat, int flags) {
   constexpr int D = M::DIM, E = M::EDIM, Z = K::ZDIM, EA = K::EADIM;
+  if (!check_quat_idxs(quat_idxs, n_quat, D)) return;   // before any stream, allocation or copy
   if (B <= 0) return;
   const long long per = D + E * E + 1 + (long long)n_obs * (Z + Z * Z + EA) + 1;
   constexpr long long PAD = 8;   // each of the six sub-buffers below is rounded up to an even number of doubles
@@ -290,7 +295,7 @@ inline void host_step(HostCtx<M>& ctx, double* x, double* P, const double* Q, co
     else cudaMemcpyAsync(dR, R + b0 * n_obs * Z * Z, sizeof(double) * nb * n_obs * Z * Z, cudaMemcpyHostToDevice, st);
     if (EA > 0 && ea) cudaMemcpyAsync(dea, ea + b0 * n_obs * EA, sizeof(double) * nb * n_obs * EA, cudaMemcpyHostToDevice, st);
     StepArgs<M::NG> a;
-    fill_common<M>(a, ctx, nb, quat_idxs, n_quat, flags);
+    fill_common<M>(a, ctx, nb, quat_idxs, n_quat, flags);   // validated above: cannot fail
     a.x = dx; a.P = dP; a.Q = dQ; a.dt_arr = dt_arr ? ddt : nullptr; a.dt = dt;
     a.z = dz; a.R = dR; a.ea = (EA > 0 && ea) ? dea : nullptr; a.ea_dim = EA; a.n_obs = n_obs;
     launch_step<M, K, true, true>(a, st);

@@ -14,7 +14,7 @@
 
 namespace rnb {
 
-constexpr int MAX_QUAT = 8;
+constexpr int MAX_QUAT = 16;   // the MSCKF normalises 11 (main state + 10 clones)
 
 // runtime flags of a batched step
 enum : int {
@@ -172,6 +172,25 @@ inline bool check(cudaError_t e, const char* what) {
   fprintf(stderr, "[rednose_b200] CUDA failure in %s: %s\n", what, cudaGetErrorString(e));
   if (getenv("REDNOSE_B200_ABORT_ON_ERROR")) abort();
   return false;
+}
+
+// The quaternion index list is copied into every launch's argument block and dereferenced in shared memory by the
+// kernels, so it is validated on the host before anything is launched: 0 <= n_quat <= MAX_QUAT and every
+// quaternion [idx, idx + 4) inside the DIM-long state.  On failure nothing runs and the status is cudaErrorInvalidValue.
+inline bool check_quat_idxs(const int* quat_idxs, int n_quat, int dim) {
+  if (n_quat < 0 || n_quat > MAX_QUAT || (n_quat > 0 && !quat_idxs)) {
+    fprintf(stderr, "[rednose_b200] n_quat = %d: at most %d quaternion indices are supported\n", n_quat, MAX_QUAT);
+    last_status() = (int)cudaErrorInvalidValue;
+    return false;
+  }
+  for (int i = 0; i < n_quat; ++i) {
+    if (quat_idxs[i] < 0 || quat_idxs[i] > dim - 4) {
+      fprintf(stderr, "[rednose_b200] quaternion index %d does not fit a state of %d entries\n", quat_idxs[i], dim);
+      last_status() = (int)cudaErrorInvalidValue;
+      return false;
+    }
+  }
+  return true;
 }
 
 

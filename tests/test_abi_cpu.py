@@ -71,6 +71,29 @@ def test_generator_features_symbols(gen_dir):
     assert hasattr(lib, sym)
 
 
+@pytest.mark.parametrize("quats", [list(range(0, 17)), [3, 20], [-1]], ids=["n_quat=MAX_QUAT+1", "idx=20", "idx=-1"])
+def test_invalid_quaternion_list_is_rejected_before_any_launch(gen_dir, quats):
+  """More than MAX_QUAT (16) quaternion indices, or a quaternion that does not fit the 23-entry state, is refused on the
+  host: a message, status cudaErrorInvalidValue (1), and no CUDA call at all (so this runs without a GPU).  Accepting
+  it would mean normalising only some quaternions or writing outside the state in shared memory."""
+  from rednose_b200.loader import load_code
+  ffi, lib = load_code(gen_dir, "live")
+  assert lib.live_cuda_status() == 0
+  x, P, Q, z, R = (ffi.new("double[]", n) for n in (23, 22 * 22, 22 * 22, 3, 9))
+  qi = ffi.new("int[]", quats)
+  n = len(quats)
+  lib.live_batch_step_12(x, P, Q, ffi.NULL, 0.01, z, R, ffi.NULL, 1, 1, qi, n, 3, ffi.NULL, ffi.NULL, ffi.NULL, ffi.NULL, ffi.NULL)
+  assert lib.live_cuda_status() == 1
+  lib.live_batch_predict(x, P, Q, ffi.NULL, 0.01, 1, qi, n, 3, ffi.NULL, ffi.NULL, ffi.NULL)
+  assert lib.live_cuda_status() == 1
+  lib.live_host_step_12(x, P, Q, ffi.NULL, 0.01, z, R, ffi.NULL, 1, 1, qi, n, 3)
+  assert lib.live_cuda_status() == 1
+  t = ffi.new("double[]", 2)
+  lib.live_batch_rts(x, P, x, P, t, 0, x, P, 2, 1, qi, n, 1, ffi.NULL)
+  assert lib.live_cuda_status() == 1
+  assert lib.live_cuda_status() == 0     # reading the status clears it
+
+
 ADAPTER_PROGRAM = r"""
 // host program of a maintainer of the reference: its own `struct EKF` (field list of rednose/helpers/ekf.h:14-33, minus
 // the Eigen include this image lacks), the adapter header of this repository, and a loader that is

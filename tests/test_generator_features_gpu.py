@@ -5,7 +5,7 @@ import os
 import numpy as np
 import pytest
 
-from tests.util import Oracle, rel_err
+from tests.util import Oracle, cov_err, state_err
 
 pytestmark = pytest.mark.gpu
 
@@ -49,7 +49,7 @@ def test_global_vars_extra_routine_and_gated_kind(dirs):
     R1 = np.tile(np.array([[1e-4]]), (B, 1, 1))
     xr, Pr, yr = o.batch_step(1, x, P, F.Q, 0.02, z1, R1)
     y = e.step(1, 0.02, z1, R1)
-    assert rel_err(e.state(), xr) < 1e-12 and rel_err(e.covs(), Pr) < 1e-10 and rel_err(y.cpu().numpy()[:, 0], yr) < 1e-10
+    assert state_err(e.state(), xr) < 1e-12 and cov_err(e.covs(), Pr) < 1e-10 and state_err(y.cpu().numpy()[:, 0], yr) < 1e-10
     # kind 2 (m = 2, extra args, Mahalanobis gated) with 20 % gross outliers
     pivot = rng.normal(0, 1.0, (B, 2))
     x2 = e.state()
@@ -60,7 +60,7 @@ def test_global_vars_extra_routine_and_gated_kind(dirs):
     z2, R2 = h + noise, np.tile(np.eye(2) * 1e-4, (B, 1, 1))
     xr2, Pr2, yr2 = o.update(2, xr, Pr, z2, R2, ea=pivot)
     y2 = e.update(2, z2, R2, ea=pivot)
-    assert rel_err(e.state(), xr2) < 1e-10 and rel_err(e.covs(), Pr2) < 1e-9 and rel_err(y2.cpu().numpy()[:, 0], yr2) < 1e-10
+    assert state_err(e.state(), xr2) < 1e-10 and cov_err(e.covs(), Pr2) < 1e-9 and state_err(y2.cpu().numpy()[:, 0], yr2) < 1e-10
     gated = np.trace(e.covs(), axis1=1, axis2=2) > np.trace(Pr, axis1=1, axis2=2) * (1 - 1e-9)
     assert gated[out].all() and gated[~out].mean() < 0.15   # gross outliers always gated; ~5 % false positives at the 0.95 quantile
   # extra routine + set_global through the drop-in driver

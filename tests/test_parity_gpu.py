@@ -1,18 +1,20 @@
 """GPU parity tests: the CUDA path (through the C-ABI) against the oracle on identical inputs.
 
-Tolerance: per-array max-norm relative error <= 1e-6 (BASELINE.json north_star, float64); the
-structured arithmetic actually agrees to ~1e-11, asserted at 1e-9 so regressions are visible.
+Metrics (tests/util.py): state_err is the worst per-component relative error of states and innovations, cov_err
+the worst covariance error in correlation units.  Tolerances are set from the errors measured on an H100 with
+about 10x headroom; TIGHT (1e-9) wherever that holds.
 """
 import numpy as np
 import pytest
 import torch
 
 from tests.test_oracle_cpu import GOLDEN, P0, Q, X0, run_kinematic_procedure
-from tests.util import LIVE_KINDS, Oracle, kinematic_batch, live_batch, live_obs, rel_err
+from tests.util import LIVE_KINDS, Oracle, cov_err, kinematic_batch, live_batch, live_obs, quat_norm_err, state_err
 
 pytestmark = pytest.mark.gpu
 TOL = 1e-6       # the contract
 TIGHT = 1e-9     # what the implementation achieves on well-conditioned inputs
+QN = 1e-15       # | |q| - 1 | after a normalising step: a few ulp
 
 
 def _engine(gen_dir, name, x, P, Qm, **kw):
@@ -53,7 +55,7 @@ def test_kinematic_batched_step(gen_dir, oracle_dir):
   xr, Pr, yr = o.batch_step(1, x, P, Qm, dt, z, R)
   e = _engine(gen_dir, "kinematic", x, P, Qm)
   y = e.step(1, torch.as_tensor(dt), z, R)
-  assert rel_err(e.state(), xr) < TIGHT and rel_err(e.covs(), Pr) < TIGHT and rel_err(y.cpu().numpy()[:, 0], yr) < TIGHT
+  assert state_err(e.state(), xr) < TIGHT and cov_err(e.covs(), Pr) < TIGHT and state_err(y.cpu().numpy()[:, 0], yr) < TIGHT
 
 
 @pytest.mark.parametrize("kind", sorted(LIVE_KINDS))
@@ -65,8 +67,9 @@ def test_live_fused_step_every_kind(gen_dir, oracle_dir, kind):
   xr, Pr, yr = o.batch_step(kind, x, P, Qm, 0.01, z, R, quat_idxs=[3], flags=3)
   e = _engine(gen_dir, "live", x, P, Qm, quaternion_idxs=[3])
   y = e.step(kind, 0.01, z, R)
-  ex, eP, ey = rel_err(e.state(), xr), rel_err(e.covs(), Pr), rel_err(y.cpu().numpy()[:, 0], yr)
+  ex, eP, ey = state_err(e.state(), xr), cov_err(e.covs(), Pr), state_err(y.cpu().numpy()[:, 0], yr)
   assert ex < TIGHT and eP < TIGHT and ey < TIGHT, (ex, eP, ey)
+  assert quat_norm_err(e.state(), [3]) <= QN
 
 
 def test_live_predict_and_update_separately(gen_dir, oracle_dir):
@@ -76,11 +79,11 @@ def test_live_predict_and_update_separately(gen_dir, oracle_dir):
   xr, Pr = o.predict(x, P, Qm, 0.02)
   e = _engine(gen_dir, "live", x, P, Qm, norm_after_predict=False, norm_after_update=False)
   e.predict(0.02)
-  assert rel_err(e.state(), xr) < TIGHT and rel_err(e.covs(), Pr) < TIGHT
+  assert state_err(e.state(), xr) < TIGHT and cov_err(e.covs(), Pr) < TIGHT
   z, R = live_obs(o, 13, xr)
   xr2, Pr2, yr = o.update(13, xr, Pr, z, R)
   y = e.update(13, z, R)
-  assert rel_err(e.state(), xr2) < TIGHT and rel_err(e.covs(), Pr2) < TIGHT and rel_err(y.cpu().numpy()[:, 0], yr) < TIGHT
+  assert state_err(e.state(), xr2) < TIGHT and cov_err(e.covs(), Pr2) < TIGHT and state_err(y.cpu().numpy()[:, 0], yr) < TIGHT
 
 
 def test_live_stream_300_steps(gen_dir, oracle_dir):
@@ -95,9 +98,10 @@ def test_live_stream_300_steps(gen_dir, oracle_dir):
     z, R = live_obs(o, kind, xr, seed=100 + k)
     xr, Pr, yr = o.batch_step(kind, xr, Pr, Qm, 0.01, z, R, quat_idxs=[3], flags=3)
     y = e.step(kind, 0.01, z, R)
-    if k in (0, 1, 50, 299):
-      assert rel_err(e.state(), xr) < TOL and rel_err(e.covs(), Pr) < TOL, k
-  assert rel_err(e.state(), xr) < 1e-8 and rel_err(e.covs(), Pr) < 1e-8
+    if k in (0, 1, 50, 299):   # measured on an H100: worst 8.1e-10 (state), 1.4e-9 (covariance)
+      assert state_err(e.state(), xr) < 1e-8 and cov_err(e.covs(), Pr) < 1e-8, k
+      assert quat_norm_err(e.state(), [3]) <= QN, k
+  assert state_err(e.state(), xr) < 1e-8 and cov_err(e.covs(), Pr) < 1e-8
 
 
 def test_multiple_observations_per_predict(gen_dir, oracle_dir):
@@ -111,7 +115,7 @@ def test_multiple_observations_per_predict(gen_dir, oracle_dir):
     xr, Pr, _ = o.update(4, xr, Pr, zs[i], Rs[i])
   e = _engine(gen_dir, "live", x, P, Qm, norm_after_predict=False, norm_after_update=False)
   e.step(4, 0.01, np.stack(zs, 1), np.stack(Rs, 1))
-  assert rel_err(e.state(), xr) < TIGHT and rel_err(e.covs(), Pr) < TIGHT
+  assert state_err(e.state(), xr) < TIGHT and cov_err(e.covs(), Pr) < TIGHT
 
 
 def test_leaf_functions_match_reference_generated_c(gen_dir, oracle_dir):
@@ -121,31 +125,40 @@ def test_leaf_functions_match_reference_generated_c(gen_dir, oracle_dir):
   kf = EKF_sym(gen_dir, "live", LiveKalman.Q, LiveKalman.initial_x, np.diag(LiveKalman.initial_P_diag), 23, 22)
   x, _, _ = live_batch(4, seed=7)
   rng = np.random.default_rng(0)
+  got, want = {}, {}     # every output entry is compared per entry, scaled by its largest value over the 4 states
+
+  def put(key, a, r):
+    got.setdefault(key, []).append(a.copy()); want.setdefault(key, []).append(r.copy())
+
   for b in range(4):
     xb = np.ascontiguousarray(x[b])
     for fn, shape, args in [("f_fun", 23, (0.01,)), ("F_fun", 22 * 22, (0.01,))]:
       a, r = np.zeros(shape), np.zeros(shape)
       getattr(kf, "f" if fn == "f_fun" else "F")(xb, 0.01, a)
       o.leaf(fn, xb, 0.01, r)
-      assert rel_err(a, r) < 1e-13, fn
+      put(fn, a, r)
     a, r = np.zeros(23 * 22), np.zeros(23 * 22)
     kf.H_mod(xb, a); o.leaf("H_mod_fun", xb, r)
-    assert rel_err(a, r) < 1e-13
+    put("H_mod_fun", a, r)
     d = rng.normal(0, 0.01, 22)
     a, r = np.zeros(23), np.zeros(23)
     kf.err_function(xb, d, a); o.leaf("err_fun", xb, d, r)
-    assert rel_err(a, r) < 1e-13
+    put("err_fun", a, r)
     a2, r2 = np.zeros(22), np.zeros(22)
     kf.inv_err_function(xb, a, a2); o.leaf("inv_err_fun", xb, r, r2)
-    assert rel_err(a2, r2) < 1e-9 and rel_err(a2, d) < 1e-3
+    put("inv_err_fun", a2, r2)
+    assert np.max(np.abs(a2 - d)) < 1e-3 * np.max(np.abs(d))     # inv_err_fun inverts err_fun to first order
     dummy = np.zeros(1)
     for k, m in LIVE_KINDS.items():
       a, r = np.zeros(m), np.zeros(m)
       kf.hs[k](xb, dummy, a); o.leaf(f"h_{k}", xb, dummy, r)
-      assert rel_err(a, r) < 1e-12, k
+      put(f"h_{k}", a, r)
       a, r = np.zeros(m * 23), np.zeros(m * 23)
       kf.Hs[k](xb, dummy, a); o.leaf(f"H_{k}", xb, dummy, r)
-      assert rel_err(a, r) < 1e-12, k
+      put(f"H_{k}", a, r)
+  for key in got:
+    err = state_err(np.stack(got[key]), np.stack(want[key]))
+    assert err < (1e-9 if key == "inv_err_fun" else 1e-13), (key, err)
 
 
 def test_host_buffer_entry_point_equals_device_path(gen_dir):
@@ -186,7 +199,7 @@ def test_full_size_properties_1m_live(gen_dir, oracle_dir):
   qn = e.x[:, 3:7].norm(dim=1)
   assert float((qn - 1).abs().max()) < 1e-14                                # quaternion normalised
   xr, Pr, yr = o.batch_step(4, x, P, Qm, 0.01, z, R, quat_idxs=[3], flags=3)
-  assert rel_err(xs[-1].cpu().numpy(), xr) < TIGHT and rel_err(Ps[-1].cpu().numpy(), Pr) < TIGHT
+  assert state_err(xs[-1].cpu().numpy(), xr) < TIGHT and cov_err(Ps[-1].cpu().numpy(), Pr) < TIGHT
   assert B == 1048576
 
 
@@ -217,9 +230,9 @@ def test_rts_smoother_matches_reference_recursion(gen_dir, oracle_dir, norm_quat
   worst_x = worst_P = 0.0
   for b in range(0, B, 4):
     xr, Pr = rts_smooth(o, hx_p[:, b], hx_f[:, b], hP_p[:, b], hP_f[:, b], t, 23, 22, norm_quats=norm_quats)
-    worst_x = max(worst_x, rel_err(xs[:, b], xr))
-    worst_P = max(worst_P, rel_err(Ps[:, b], Pr))
-  assert worst_x < TOL and worst_P < TOL, (worst_x, worst_P)
+    worst_x = max(worst_x, state_err(xs[:, b], xr))
+    worst_P = max(worst_P, cov_err(Ps[:, b], Pr))
+  assert worst_x < TIGHT and worst_P < TIGHT, (worst_x, worst_P)
   # smoothing must not increase the position variance of interior points
   assert np.all(Ps[5, :, 0, 0] <= hP_f[5, :, 0, 0] * (1 + 1e-9))
 
@@ -248,15 +261,17 @@ def test_cuda_path_reproduces_reference_golden_vectors(gen_dir):
     z = np.stack([g[f"z{b}"][k, :m] for b in range(2)])
     R = np.stack([g[f"R{b}"][k, :m, :m] for b in range(2)])
     y = e.step_recorded(hist, int(kind), float(ts[k]), z, R).cpu().numpy()[:, 0]
-    for b in range(2):
-      assert rel_err(e.state()[b], g[f"x_filt{b}"][k]) < 1e-9, (b, k, kind)
-      assert rel_err(e.covs()[b], g[f"P_filt{b}"][k]) < 1e-8, (b, k, kind)
-      assert np.max(np.abs(y[b] - g[f"y{b}"][k, :m])) < 1e-6 * max(1.0, np.max(np.abs(g[f"y{b}"][k, :m])))
+    ex = state_err(e.state(), np.stack([g[f"x_filt{b}"][k] for b in range(2)]))
+    eP = cov_err(e.covs(), np.stack([g[f"P_filt{b}"][k] for b in range(2)]))
+    assert ex < TIGHT and eP < TIGHT, (k, kind, ex, eP)
+    assert quat_norm_err(e.state(), [3]) <= QN
+    ey = state_err(y, np.stack([g[f"y{b}"][k, :m] for b in range(2)]))
+    assert ey < TIGHT, (k, kind, ey)
   for b in range(2):
-    assert rel_err(hist.P_pred[:, b].cpu().numpy(), g[f"P_pred{b}"]) < 1e-8
+    assert cov_err(hist.P_pred[:, b].cpu().numpy(), g[f"P_pred{b}"]) < TIGHT
   xs, Ps = e.rts_smooth(hist, norm_quats=True)
   for b in range(2):
-    assert rel_err(xs[:, b].cpu().numpy(), g[f"xs{b}"]) < TOL and rel_err(Ps[:, b].cpu().numpy(), g[f"Ps{b}"]) < TOL
+    assert state_err(xs[:, b].cpu().numpy(), g[f"xs{b}"]) < TIGHT and cov_err(Ps[:, b].cpu().numpy(), g[f"Ps{b}"]) < TIGHT
 
 
 def test_shared_R_equals_replicated_R(gen_dir):
@@ -330,7 +345,8 @@ def test_ragged_scheduler_matches_per_filter_driving(gen_dir, oracle_dir):
       t_ref[sel] = t_obs[kinds == k]
     sch.tick(active, t_obs, kinds, zs, Rs)
   assert sch.dropped == 0
-  assert rel_err(e.state(), xr) < TIGHT and rel_err(e.covs(), Pr) < TIGHT
+  assert state_err(e.state(), xr) < TIGHT and cov_err(e.covs(), Pr) < TIGHT
+  assert quat_norm_err(e.state(), [3]) <= QN
   assert np.allclose(sch.t_filter.cpu().numpy(), t_ref, equal_nan=True)
   # a late observation is dropped, not applied
   before = e.state().copy()
@@ -350,7 +366,7 @@ def test_edge_batches_empty_single_and_ragged_tail(gen_dir, oracle_dir):
     assert y.shape[0] == B
     if B:
       xr, Pr, yr = o.batch_step(12, x, P, Qm, 0.01, z, R, quat_idxs=[3], flags=3)
-      assert rel_err(e.state(), xr) < TIGHT and rel_err(e.covs(), Pr) < TIGHT
+      assert state_err(e.state(), xr) < TIGHT and cov_err(e.covs(), Pr) < TIGHT
 
 
 def test_tiled_smoother_equals_untiled(gen_dir, oracle_dir):
@@ -397,7 +413,7 @@ def test_batched_maha_query_matches_reference_formula(gen_dir, oracle_dir):
       He = H.reshape(m, 23) @ Hm.reshape(23, 22)
       y = z[b] - h
       want[b] = y @ np.linalg.inv(He @ P[b] @ He.T + R[b]) @ y
-    assert rel_err(d, want) < 1e-9, kind
+    assert state_err(d[:, None], want[:, None]) < 1e-9, kind
     assert torch.equal(e.x.cpu(), torch.as_tensor(x))   # a query: state untouched
     passed = e.maha_test(kind, z, R).cpu().numpy()
     from rednose_b200.chi2 import chi2_ppf
@@ -423,7 +439,7 @@ def test_batched_kalmanfilter_front_end(gen_dir, oracle_dir):
   kf.predict_and_observe(0.05, 1, z)
   xr, Pr, _ = o.batch_step(1, x, P, Qm, 0.0, z, R)
   xr, Pr, _ = o.batch_step(1, xr, Pr, Qm, 0.05, z, R)
-  assert rel_err(kf.x, xr) < TIGHT and rel_err(kf.P, Pr) < TIGHT and kf.t == 0.05
+  assert state_err(kf.x, xr) < TIGHT and cov_err(kf.P, Pr) < TIGHT and kf.t == 0.05
   assert kf.maha_test(1, z).shape == (B,)
 
 
@@ -438,7 +454,7 @@ def test_gather_list_on_the_thread_kernel(gen_dir, oracle_dir):
   e.step_indexed(1, idx, dt, z[sel], R[sel])
   xr, Pr, _ = o.batch_step(1, x[sel], P[sel], Qm, dt.numpy(), z[sel], R[sel])
   gx, gP = e.state(), e.covs()
-  assert rel_err(gx[sel], xr) < TIGHT and rel_err(gP[sel], Pr) < TIGHT
+  assert state_err(gx[sel], xr) < TIGHT and cov_err(gP[sel], Pr) < TIGHT
   keep = np.setdiff1d(np.arange(B), sel)
   assert np.array_equal(gx[keep], x[keep]) and np.array_equal(gP[keep], P[keep])
 
@@ -457,8 +473,9 @@ def test_live_long_stream_2000_steps(gen_dir, oracle_dir):
     xr, Pr, _ = o.batch_step(kind, xr, Pr, Qm, 0.01, z, R, quat_idxs=[3], flags=3, nthreads=1)
     e.step(kind, 0.01, z, R)
     if k % 250 == 249:
-      worst = max(worst, rel_err(e.state(), xr), rel_err(e.covs(), Pr))
-  assert worst < 1e-7, worst
+      worst = max(worst, state_err(e.state(), xr), cov_err(e.covs(), Pr))
+      assert quat_norm_err(e.state(), [3]) <= QN
+  assert worst < 2e-8, worst       # measured on an H100: 1.8e-9
 
 
 def test_rts_scalar_fallback_on_the_kinematic_model(gen_dir, oracle_dir):
@@ -480,7 +497,7 @@ def test_rts_scalar_fallback_on_the_kinematic_model(gen_dir, oracle_dir):
   t = hist.t_host.copy()
   for b in range(0, B, 7):
     xr, Pr = rts_smooth(o, hx_p[:, b], hx_f[:, b], hP_p[:, b], hP_f[:, b], t, 2, 2)
-    assert rel_err(xs[:, b], xr) < 1e-9 and rel_err(Ps[:, b], Pr) < 1e-9
+    assert state_err(xs[:, b], xr) < 1e-9 and cov_err(Ps[:, b], Pr) < 1e-9
 
 
 @pytest.fixture
@@ -514,7 +531,7 @@ def test_pair_and_single_kernels_agree_to_rounding(gen_dir, oracle_dir, monkeypa
     e = _engine(gen_dir, "live", x, P, Qm, quaternion_idxs=[3])
     y = e.step(10, 0.01, z, R)
     out.append((e.state().copy(), e.covs().copy(), y.cpu().numpy().copy()))
-  assert rel_err(out[0][0], out[1][0]) < 1e-14 and rel_err(out[0][1], out[1][1]) < 1e-14 and rel_err(out[0][2], out[1][2]) < 1e-14
+  assert state_err(out[0][0], out[1][0]) < 1e-14 and cov_err(out[0][1], out[1][1]) < 1e-14 and state_err(out[0][2], out[1][2]) < 1e-14
 
 
 def test_dense_process_noise(gen_dir, oracle_dir):
@@ -529,7 +546,7 @@ def test_dense_process_noise(gen_dir, oracle_dir):
   xr, Pr, yr = o.batch_step(4, x, P, Qd, 0.01, z, R, quat_idxs=[3], flags=3)
   e = _engine(gen_dir, "live", x, P, Qd, quaternion_idxs=[3])
   y = e.step(4, 0.01, z, R)
-  assert rel_err(e.state(), xr) < TIGHT and rel_err(e.covs(), Pr) < TIGHT and rel_err(y.cpu().numpy()[:, 0], yr) < TIGHT
+  assert state_err(e.state(), xr) < TIGHT and cov_err(e.covs(), Pr) < TIGHT and state_err(y.cpu().numpy()[:, 0], yr) < TIGHT
 
 
 def test_live_single_filter_dropin_path(gen_dir, oracle_dir):
@@ -554,7 +571,8 @@ def test_live_single_filter_dropin_path(gen_dir, oracle_dir):
         kind, data = (K.PHONE_GYRO if k % 2 else K.PHONE_ACCEL), [rng.normal(0, 0.01, 3) + (0.0 if k % 2 else np.array([0, 0, -9.8]))]
       rg, rc = gpu.predict_and_observe(t, kind, data), cpu.predict_and_observe(t, kind, data)
       assert rg is not None and rc is not None
-      assert rel_err(gpu.x, cpu.x) < TOL and rel_err(gpu.P, cpu.P) < TOL, (k, int(kind))   # contract: 1e-6
+      # measured on an H100: worst 1.1e-9 (state), 2.4e-10 (covariance)
+      assert state_err(gpu.x, cpu.x) < 1e-8 and cov_err(gpu.P, cpu.P) < 1e-8, (k, int(kind))
 
 
 def test_rewinding_scheduler_on_the_device(gen_dir, oracle_dir, monkeypatch):
@@ -594,8 +612,10 @@ def test_rewinding_scheduler_on_the_device(gen_dir, oracle_dir, monkeypatch):
     if ids:
       s.tick(np.array(ids), np.array(ts), np.array(ks), {k: np.array(v) for k, v in zs.items() if v}, Rk)
   assert s.dropped == ref_dropped and s.rewinds > 10 and s.replayed > s.rewinds
+  ex = state_err(e.state(), np.stack([r.state() for r in refs]))
+  eP = cov_err(e.covs(), np.stack([r.covs() for r in refs]))
+  assert ex < 2e-9 and eP < 2e-9, (ex, eP)     # measured on an H100: 1.8e-10, 1.7e-10
   for b in range(B):
-    assert rel_err(e.state()[b], refs[b].state()) < TOL and rel_err(e.covs()[b], refs[b].covs()) < TOL, b
     assert int(s.cnt[b]) == len(refs[b].rewind_t) and abs(float(s.t_filter[b]) - refs[b].filter_time) < 1e-12
 
 
@@ -623,9 +643,10 @@ def test_msckf_cuda_path_reproduces_reference_golden_vectors(gen_dir):
     t_prev = float(g["t"][k])
     if g["augment"][k]:
       e.augment()
-    for b in range(2):
-      ex, eP = rel_err(e.state()[b], g[f"xk{b}"][k]), rel_err(e.covs()[b], g[f"Pk{b}"][k])
-      assert ex < 1e-8 and eP < TOL, (b, k, kind, ex, eP)
+    ex = state_err(e.state(), np.stack([g[f"xk{b}"][k] for b in range(2)]))
+    eP = cov_err(e.covs(), np.stack([g[f"Pk{b}"][k] for b in range(2)]))
+    assert ex < TIGHT and eP < TIGHT, (k, kind, ex, eP)
+    assert quat_norm_err(e.state(), quats) <= QN, k          # the main quaternion and all 10 clones
 
 
 @pytest.mark.parametrize("norm_quats", [False, True])
@@ -691,8 +712,8 @@ def test_tiled_smoother_two_passes_equal_two_oracle_passes(gen_dir, oracle_dir):
   ts_ = TiledSmoother(gen_dir, "live", Qm, 23, 22, quaternion_idxs=[3], tile=8)
   ts_.run(x, P, T, lambda k, lo, hi: (ts[k], kinds[k], zs[k][0][lo:hi].copy(), zs[k][1][lo:hi]),
           lambda lo, hi, xs, Ps: got.update(a=(xs.cpu().numpy().copy(), Ps.cpu().numpy().copy())), norm_quats=True, passes=2)
-  assert rel_err(got["a"][0], xs2) < TOL and rel_err(got["a"][1], Ps2) < TOL
-  assert rel_err(xs2, xs1) > 1e-9                                        # the second pass did change the estimate
+  assert state_err(got["a"][0], xs2) < TIGHT and cov_err(got["a"][1], Ps2) < TIGHT
+  assert state_err(xs2, xs1) > 1e-9                                        # the second pass did change the estimate
 
 
 def test_rts_on_an_ill_conditioned_history(gen_dir, oracle_dir):
@@ -719,9 +740,9 @@ def test_rts_on_an_ill_conditioned_history(gen_dir, oracle_dir):
   worst_x = worst_P = 0.0
   for b in range(B):
     xr, Pr = rts_smooth(o, hx_p[:, b], hx_f[:, b], hP_p[:, b], hP_f[:, b], hist.t_host.copy(), 23, 22, norm_quats=True)
-    worst_x, worst_P = max(worst_x, rel_err(xs[:, b], xr)), max(worst_P, rel_err(Ps[:, b], Pr))
+    worst_x, worst_P = max(worst_x, state_err(xs[:, b], xr)), max(worst_P, cov_err(Ps[:, b], Pr))
   print(f"ill-conditioned RTS (cond {cond:.1e}): x {worst_x:.2e} P {worst_P:.2e}")
-  assert worst_x < 1e-5 and worst_P < 1e-5, (worst_x, worst_P)
+  assert worst_x < TIGHT and worst_P < TIGHT, (worst_x, worst_P)   # measured on an H100: 5.4e-11, 1.2e-10
   assert np.isfinite(Ps).all() and np.all(np.diagonal(Ps, axis1=2, axis2=3) > 0)
 
 
@@ -740,7 +761,7 @@ def test_full_size_1m_kinematic_sampled_oracle(gen_dir, oracle_dir):
     e.step(1, 0.01, torch.as_tensor(z).cuda(), Rd)
     xr, Pr, _ = o.batch_step(1, xr, Pr, Qm, 0.01, z[sel], R[sel])
   gx, gP = e.state(), e.covs()
-  assert rel_err(gx[sel], xr) < TIGHT and rel_err(gP[sel], Pr) < TIGHT
+  assert state_err(gx[sel], xr) < TIGHT and cov_err(gP[sel], Pr) < TIGHT
   assert np.isfinite(gx).all() and np.all(gP[:, 0, 0] > 0) and np.all(gP[:, 1, 1] > 0)
   assert float(np.max(np.abs(gP[:, 0, 1] - gP[:, 1, 0]))) < 1e-12
 

@@ -9,11 +9,40 @@ LIVE_R = {3: [0.2**2], 4: [0.025**2] * 3, 9: [0.00025**2] * 3, 10: [0.5**2] * 3,
           13: [0.1**2] * 3, 14: [0.05**2] * 3, 19: [0.05**2] * 3}
 
 
-def rel_err(a, b):
-  """Per-array max-norm relative error (SURVEY.md section 7, hard part 4)."""
-  a, b = np.asarray(a, dtype=np.float64), np.asarray(b, dtype=np.float64)
-  denom = np.max(np.abs(b))
-  return float(np.max(np.abs(a - b)) / (denom if denom > 0 else 1.0))
+def state_err(got, want, per_component=False):
+  """Worst per-component relative error of states / innovations / history slabs [..., n].
+
+  For every last-axis component i: max |got - want| over all leading axes, divided by max |want[..., i]| over the
+  same axes (absolute where the reference component is identically zero).  A 4e6 m position no longer sets the scale
+  of a unit quaternion or a 1e-2 accelerometer bias.  per_component=True returns the [n] vector instead of its max."""
+  got, want = np.asarray(got, dtype=np.float64), np.asarray(want, dtype=np.float64)
+  assert got.shape == want.shape, (got.shape, want.shape)
+  n = want.shape[-1] if want.ndim else 1
+  d = np.abs(got - want).reshape(-1, n).max(axis=0)
+  s = np.abs(want).reshape(-1, n).max(axis=0)
+  e = np.where(s > 0, d / np.where(s > 0, s, 1.0), d)
+  return e if per_component else float(np.max(e))
+
+
+def cov_err(got, want, per_component=False):
+  """Worst covariance error in correlation units: max |got_ij - want_ij| / sqrt(want_ii want_jj) per matrix [..., n, n].
+
+  Invariant under a rescaling of the state units (D P D for a positive diagonal D), so a 1e-4 variance block is held
+  to the same standard as the 1e8 position block.  per_component=True returns the [n, n] maximum over the leading axes."""
+  got, want = np.asarray(got, dtype=np.float64), np.asarray(want, dtype=np.float64)
+  assert got.shape == want.shape and want.shape[-1] == want.shape[-2], (got.shape, want.shape)
+  dg = np.diagonal(want, axis1=-2, axis2=-1)
+  assert np.all(dg > 0), "reference covariance has a non-positive diagonal entry"
+  sd = np.sqrt(dg)
+  e = np.abs(got - want) / (sd[..., :, None] * sd[..., None, :])
+  n = want.shape[-1]
+  return e.reshape(-1, n, n).max(axis=0) if per_component else float(np.max(e))
+
+
+def quat_norm_err(x, idxs):
+  """max | |q| - 1 | over every quaternion x[..., i:i + 4], i in idxs, and every filter / step."""
+  x = np.asarray(x, dtype=np.float64)
+  return float(max(np.max(np.abs(np.linalg.norm(x[..., i:i + 4], axis=-1) - 1.0)) for i in idxs))
 
 
 def live_batch(B, seed=0, well_conditioned=True):
