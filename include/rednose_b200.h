@@ -17,6 +17,10 @@
  *     void <name>_batch_predict(...), <name>_batch_update_<kind>(...), <name>_batch_step_<kind>(...)
  *     void <name>_batch_rts(...)   RTS smoother over a time-major history [T, B, ...]  (ekf_sym.py:651-690)
  *   batched, HOST pointers (copies inside): <name>_host_step_<kind>(...)
+ *   packed covariance layout (int results, so the reference's `void ` prototype set is unchanged):
+ *     int <name>_packed_P_doubles(void)   doubles per filter of the packed layout, 0 where it is not used
+ *     int <name>_convert_P(double *full, double *packed, const int *idx, long long n, int to_packed, void *stream)
+ *         full [n, EDIM, EDIM] entry e <-> packed filter idx[e] (e when idx is NULL); returns the cudaError_t
  *
  * All functions return void like the reference; CUDA failures are printed to stderr and
  * latched: `int <name>_cuda_status(void)` returns and clears the last cudaError_t (0 = ok).
@@ -36,6 +40,9 @@ extern "C" {
 #define REDNOSE_NORM_AFTER_UPDATE 2
 #define REDNOSE_Q_IS_DIAGONAL 4      /* caller promises Q is diagonal: kernels read only its diagonal */
 #define REDNOSE_SHARED_R 8           /* R is one [ZDIM, ZDIM] matrix shared by the whole batch (what get_R builds, kalmanfilter.py:37-43) */
+/* P is [B, <name>_packed_P_doubles()] in the two-filters-per-warp kernel's packed lower-block-triangle layout
+   (rednose_b200/csrc/ekf_packed.cuh); refused (cudaErrorNotSupported) wherever that kernel does not serve the launch */
+#define REDNOSE_PACKED_P 32
 
 typedef void (*rednose_leaf3_fn)(double *, double *, double *);
 typedef void (*rednose_leaf2_fn)(double *, double *);

@@ -8,6 +8,10 @@ the generated library's fused ``<name>_batch_step_<kind>`` kernel through its C-
 
 Semantics follow the C++ driver: predict(dt) -> [normalise quaternions] -> update(kind) ->
 [normalise] (ekf_sym.cc:162,207,213); the innovation overwrites ``z`` (ekf_c.c:120).
+
+Filters served by the two-filters-per-warp kernel (even EDIM <= 32, e.g. live_kf) keep P resident in that kernel's packed
+layout, the lower block triangle of 2x2 blocks (csrc/ekf_packed.cuh: 264 instead of 484 doubles per live filter), which
+halves the covariance traffic of a step.  ``P`` still reads as the full ``[B, EDIM, EDIM]`` tensor; see ``BatchedEKF.P``.
 """
 from __future__ import annotations
 
@@ -21,6 +25,7 @@ NORM_AFTER_UPDATE = 2
 Q_IS_DIAGONAL = 4
 SHARED_R = 8
 AUGMENT = 16   # fused clone-window shift (CTA kernel only)
+PACKED_P = 32  # P is in the packed lower-block-triangle layout (two-filters-per-warp kernel only)
 
 
 def _as_device(t, device, dtype=torch.float64):
@@ -50,7 +55,16 @@ class BatchedEKF:
       P0 = P0.expand(B, -1, -1)
     self.B, self.dim_x, self.dim_err = B, x0.shape[1], P0.shape[1]
     self.x = x0.contiguous().clone()
-    self.P = P0.contiguous().clone()
+    # covariance storage: the full buffer `_Pf` and, when the pair kernel serves this filter, the packed resident buffer
+    # `_Pk`; `_full_owns` says which of the two holds the current P
+    self._packed_doubles = int(getattr(self._lib, f"{name}_packed_P_doubles")())
+    self._Pf = P0.contiguous().clone()
+    self._full_owns = True
+    self._Pk = None
+    if self._packed_doubles:
+      self._Pk = torch.empty(B, self._packed_doubles, dtype=torch.float64, device=self.device)
+      self._sync_packed()
+      self._Pf = None            # a million live covariances are 3.9 GB in full: allocated again only when P is read
     self.Q = _as_device(Q, self.device)
     assert self.Q.shape == (self.dim_err, self.dim_err)
     self.filter_time = None  # scalar time shared by the batch, or a [B] tensor
@@ -65,6 +79,67 @@ class BatchedEKF:
     self.launches = 0  # kernels launched through this object (bench.py reports it)
     for g, v in (global_vars or {}).items():
       getattr(self._lib, f"{name}_set_{g}")(float(v))
+
+  # -------------------------------------------------------------- covariance ---
+  @property
+  def P(self):
+    """The covariances as a [B, EDIM, EDIM] tensor.  With the packed resident layout this unpacks into a full buffer
+    that is kept allocated; from then on that buffer is the state (the caller may write through it), and the next step
+    packs it again.  So a handle taken from ``P`` is a snapshot of the moment it was read, not live storage: read ``P``
+    again after stepping."""
+    if self._Pk is not None and not self._full_owns:
+      if self._Pf is None:
+        self._Pf = torch.empty(self.B, self.dim_err, self.dim_err, dtype=torch.float64, device=self.device)
+      self._convert(self._Pf, None, self.B, to_packed=False)
+      self._full_owns = True
+    return self._Pf
+
+  @P.setter
+  def P(self, value):
+    value = _as_device(value, self.device)
+    assert value.shape == (self.B, self.dim_err, self.dim_err)
+    self._Pf = value
+    self._full_owns = True
+
+  def _convert(self, full, idx, n, to_packed):
+    with torch.cuda.device(self.device):
+      getattr(self._lib, f"{self.name}_convert_P")(
+        self._p(full), self._p(self._Pk), self._ffi.cast("const int *", idx.data_ptr()) if idx is not None else self._ffi.NULL,
+        int(n), 1 if to_packed else 0, self._stream())
+    self._check("convert_P")
+
+  def _sync_packed(self):
+    if self._full_owns:
+      self._convert(self._Pf, None, self.B, to_packed=True)
+      self._full_owns = False
+
+  def _P_arg(self):
+    """(pointer to the covariance a launch reads and writes, layout flag)."""
+    if self._Pk is None:
+      return self._p(self._Pf), 0
+    self._sync_packed()
+    return self._p(self._Pk), PACKED_P
+
+  def get_P_rows(self, ids):
+    """P of the filters `ids` as a new [n, EDIM, EDIM] tensor, without converting the rest of the batch."""
+    ids = torch.as_tensor(ids, device=self.device)
+    if self._Pk is None or self._full_owns:
+      return self._Pf[ids]
+    out = torch.empty(int(ids.shape[0]), self.dim_err, self.dim_err, dtype=torch.float64, device=self.device)
+    if out.shape[0]:
+      self._convert(out, ids.to(torch.int32).contiguous(), out.shape[0], to_packed=False)
+    return out
+
+  def set_P_rows(self, ids, P):
+    """Overwrite P of the filters `ids` (distinct) with P [n, EDIM, EDIM]; only their lower triangles are kept in the
+    packed layout."""
+    ids = torch.as_tensor(ids, device=self.device)
+    if self._Pk is None or self._full_owns:
+      self._Pf[ids] = P
+      return
+    P = _as_device(P, self.device)
+    if P.shape[0]:
+      self._convert(P, ids.to(torch.int32).contiguous(), P.shape[0], to_packed=True)
 
   # ----------------------------------------------------------------- helpers ---
   def _p(self, t):
@@ -91,9 +166,10 @@ class BatchedEKF:
     """P <- F P F^T + dt Q, x <- f(x, dt) for the whole batch (ekf_c.c:8-33)."""
     keep, dt_ptr, dt_s = self._dt_args(dt)
     hx, hP = (hist if hist is not None else (None, None))
+    P, pflag = self._P_arg()
     with torch.cuda.device(self.device):
       getattr(self._lib, f"{self.name}_batch_predict")(
-        self._p(self.x), self._p(self.P), self._cp(self.Q), dt_ptr, dt_s, self.B, self._quat, self._nquat, self.flags,
+        self._p(self.x), P, self._cp(self.Q), dt_ptr, dt_s, self.B, self._quat, self._nquat, self.flags | pflag,
         self._p(hx), self._p(hP), self._stream())
     self.launches += 1
     self._check("batch_predict")
@@ -119,10 +195,11 @@ class BatchedEKF:
     """Measurement update of one kind for the whole batch (ekf_c.c:37-121); returns the innovations y [B, n, m]."""
     z, R, ea, n_obs, flags = self._obs_args(z, R, ea)
     hx, hP = (hist if hist is not None else (None, None))
+    P, pflag = self._P_arg()
     with torch.cuda.device(self.device):
       getattr(self._lib, f"{self.name}_batch_update_{kind}")(
-        self._p(self.x), self._p(self.P), self._p(z), self._cp(R), self._cp(ea), n_obs, self.B,
-        self._quat, self._nquat, flags, self._p(hx), self._p(hP), self._stream())
+        self._p(self.x), P, self._p(z), self._cp(R), self._cp(ea), n_obs, self.B,
+        self._quat, self._nquat, flags | pflag, self._p(hx), self._p(hP), self._stream())
     self.launches += 1
     self._check(f"batch_update_{kind}")
     return z
@@ -152,10 +229,11 @@ class BatchedEKF:
       dt_ptr, dt_s = self._cp(dt), 0.0
     else:
       dt_ptr, dt_s = self._ffi.NULL, float(dt)
+    P, pflag = self._P_arg()
     with torch.cuda.device(self.device):
       getattr(self._lib, f"{self.name}_batch_step_{kind}_idx")(
-        self._p(self.x), self._p(self.P), self._cp(self.Q), dt_ptr, dt_s, self._p(z), self._cp(R), self._cp(ea),
-        z.shape[1], n, self._quat, self._nquat, flags, self._ffi.NULL, self._ffi.NULL, self._ffi.NULL, self._ffi.NULL,
+        self._p(self.x), P, self._cp(self.Q), dt_ptr, dt_s, self._p(z), self._cp(R), self._cp(ea),
+        z.shape[1], n, self._quat, self._nquat, flags | pflag, self._ffi.NULL, self._ffi.NULL, self._ffi.NULL, self._ffi.NULL,
         self._ffi.cast("const int *", idx.data_ptr()), self._stream())
     self.launches += 1
     self._check(f"batch_step_{kind}_idx")
@@ -172,10 +250,11 @@ class BatchedEKF:
       flags |= AUGMENT
     hxp, hPp = (hist_pred if hist_pred is not None else (None, None))
     hxf, hPf = (hist_filt if hist_filt is not None else (None, None))
+    P, pflag = self._P_arg()
     with torch.cuda.device(self.device):
       getattr(self._lib, f"{self.name}_batch_step_{kind}")(
-        self._p(self.x), self._p(self.P), self._cp(self.Q), dt_ptr, dt_s, self._p(z), self._cp(R), self._cp(ea),
-        n_obs, self.B, self._quat, self._nquat, flags, self._p(hxp), self._p(hPp), self._p(hxf), self._p(hPf),
+        self._p(self.x), P, self._cp(self.Q), dt_ptr, dt_s, self._p(z), self._cp(R), self._cp(ea),
+        n_obs, self.B, self._quat, self._nquat, flags | pflag, self._p(hxp), self._p(hPp), self._p(hxf), self._p(hPf),
         self._stream())
     self.launches += 1
     self._check(f"batch_step_{kind}")
@@ -201,17 +280,28 @@ class BatchedEKF:
     allocations) -- into a CUDA graph and return it; `graph.replay()` then re-issues the whole sequence with one driver
     call.  For small states (kinematic: 28 us per launch of a million filters) the per-launch driver cost is comparable
     to the kernel, and a captured loop removes it.  `fn` is run `warmup` times first, uncaptured, so that one-time kernel
-    attribute setup does not land inside the capture."""
+    attribute setup does not land inside the capture.
+
+    With the packed resident layout the graph packs ``P`` before the captured launches and unpacks it after them, so a
+    replay reads and writes the full ``P`` a caller sees (``eng.P.copy_(P0); graph.replay()`` restarts from P0)."""
     side = torch.cuda.Stream(self.device)
     side.wait_stream(torch.cuda.current_stream(self.device))
     with torch.cuda.stream(side):
       for _ in range(max(1, int(warmup))):
         fn()
+      if self._Pk is not None:
+        self.P                # the full buffer exists and holds the current state before the capture starts
     torch.cuda.current_stream(self.device).wait_stream(side)
     g = torch.cuda.CUDAGraph()
     with torch.cuda.graph(g, stream=side):
+      if self._Pk is not None:
+        self._convert(self._Pf, None, self.B, to_packed=True)
+        self._full_owns = False
       fn()
-    return g
+      if self._Pk is not None:
+        self._convert(self._Pf, None, self.B, to_packed=False)
+        self._full_owns = True
+    return g if self._Pk is None else _PackedGraph(g, self)
 
   # -------------------------------------------------------------- host access ---
   def state(self):
@@ -222,7 +312,10 @@ class BatchedEKF:
 
   def init_state(self, x, P, filter_time=None):
     self.x.copy_(_as_device(x, self.device).expand_as(self.x))
-    self.P.copy_(_as_device(P, self.device).expand_as(self.P))
+    if self._Pf is None:
+      self._Pf = torch.empty(self.B, self.dim_err, self.dim_err, dtype=torch.float64, device=self.device)
+    self._Pf.copy_(_as_device(P, self.device).expand_as(self._Pf))   # overwrites every filter: nothing to unpack first
+    self._full_owns = True
     self.filter_time = filter_time
 
   def maha_dist(self, kind, z, R, ea=None):
@@ -233,9 +326,10 @@ class BatchedEKF:
     flags = SHARED_R if R.ndim == 2 else 0
     ea = _as_device(ea, self.device) if ea is not None else None
     out = torch.empty(self.B, dtype=torch.float64, device=self.device)
+    P, pflag = self._P_arg()
     with torch.cuda.device(self.device):
       getattr(self._lib, f"{self.name}_batch_maha_{kind}")(
-        self._cp(self.x), self._cp(self.P), self._cp(z), self._cp(R), self._cp(ea), self.B, flags, self._p(out), self._stream())
+        self._cp(self.x), P, self._cp(z), self._cp(R), self._cp(ea), self.B, flags | pflag, self._p(out), self._stream())
     self.launches += 1
     self._check(f"batch_maha_{kind}")
     return out
@@ -249,7 +343,7 @@ class BatchedEKF:
   def augment(self):
     """MSCKF clone window shift for the whole batch (ekf_sym.py:365-391), one launch."""
     with torch.cuda.device(self.device):
-      getattr(self._lib, f"{self.name}_batch_augment")(self._p(self.x), self._p(self.P), self.B, self._stream())
+      getattr(self._lib, f"{self.name}_batch_augment")(self._p(self.x), self._p(self.P), self.B, self._stream())   # EDIM > 32: never packed
     self.launches += 1
     self._check("batch_augment")
 
@@ -306,6 +400,23 @@ class BatchedEKF:
     self.launches += 1
     self._check("batch_rts")
     return xs[:T], Ps[:T]
+
+
+class _PackedGraph:
+  """A captured graph of an engine with packed resident P: the graph reads and writes the full buffer, so before a
+  replay that buffer is brought up to date (a no-op unless the engine was stepped eagerly since), and after it the full
+  buffer holds the state."""
+
+  def __init__(self, graph, engine):
+    self.graph, self._e = graph, engine
+
+  def replay(self):
+    self._e.P                 # noqa: B018 -- unpacks only if eager steps ran since the last replay
+    self.graph.replay()
+    self._e._full_owns = True
+
+  def __getattr__(self, name):
+    return getattr(self.graph, name)
 
 
 class History:

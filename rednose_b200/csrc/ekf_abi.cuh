@@ -82,8 +82,31 @@ struct HostCtx {
 
 constexpr int THREAD_MAX_EDIM = 6;
 
+// true when a step of filter M serves its covariance with the pair kernel (ekf_warp2.cuh), the only kernel that reads
+// and writes the packed layout; reads REDNOSE_B200_WARP_KERNEL at call time, like launch_step
+template <class M>
+inline bool pair_serves() {
+  if constexpr (M::EDIM > THREAD_MAX_EDIM && use_pair<M>()) return pair_enabled();
+  else return false;
+}
+
+// doubles per filter of the packed covariance layout, 0 when the pair kernel does not serve this filter
+template <class M>
+inline int packed_P_doubles() { return pair_serves<M>() ? packed_doubles(M::EDIM) : 0; }
+
+// FLAG_PACKED_P on a launch that the pair kernel would not run: rejected before any CUDA call
+template <class M, bool FEATURE_KIND>
+inline bool check_packed_flag(int flags, const char* what) {
+  if (!(flags & FLAG_PACKED_P) || (!FEATURE_KIND && pair_serves<M>())) return true;
+  fprintf(stderr, "[rednose_b200] %s: the packed covariance layout exists only for the two-filters-per-warp kernel "
+                  "(even EDIM <= 32, no feature kinds, REDNOSE_B200_WARP_KERNEL != single)\n", what);
+  last_status() = (int)cudaErrorNotSupported;
+  return false;
+}
+
 template <class M, class K, bool PRED, bool UPD>
 inline void launch_step(const StepArgs<M::NG>& a, cudaStream_t st) {
+  if (!check_packed_flag<M, K::HAS_HE>(a.flags, "ekf_step")) return;
   if (a.B <= 0) return;
   if ((a.flags & FLAG_AUGMENT) && !(M::EDIM > 32 || K::HAS_HE)) {
     fprintf(stderr, "[rednose_b200] the fused augment exists only in the CTA-per-filter kernel (EDIM > 32): call <name>_batch_augment\n");
@@ -120,16 +143,17 @@ inline void launch_step(const StepArgs<M::NG>& a, cudaStream_t st) {
         }
         kern<<<grid, 32, smem, st>>>(a);
       };
+      const bool packed = a.flags & FLAG_PACKED_P;
       if constexpr (PRED && UPD) {
-        if (a.idx) run(ekf_step_pair<M, K, PRED, UPD, G, true>);
-        else run(ekf_step_pair<M, K, PRED, UPD, G, false>);
+        if (a.idx) run(packed ? ekf_step_pair<M, K, PRED, UPD, G, true, true> : ekf_step_pair<M, K, PRED, UPD, G, true, false>);
+        else run(packed ? ekf_step_pair<M, K, PRED, UPD, G, false, true> : ekf_step_pair<M, K, PRED, UPD, G, false, false>);
       } else {
         if (a.idx) {
           fprintf(stderr, "[rednose_b200] gather lists are only supported by the fused predict+update step\n");
           last_status() = (int)cudaErrorNotSupported;
           return;
         }
-        run(ekf_step_pair<M, K, PRED, UPD, G, false>);
+        run(packed ? ekf_step_pair<M, K, PRED, UPD, G, false, true> : ekf_step_pair<M, K, PRED, UPD, G, false, false>);
       }
     }
     if (!paired) {
@@ -212,6 +236,7 @@ namespace rnb {
 template <class M, class K>
 inline void batch_maha(HostCtx<M>& ctx, const double* x, const double* P, const double* z, const double* R, const double* ea,
                        long long B, int flags, double* out, void* stream) {
+  if (!check_packed_flag<M, false>(flags, "batch_maha")) return;
   if (B <= 0) return;
   // per-call scratch, allocated and released in stream order (no buffer shared between streams or devices)
   double* scratch = (double*)stream_alloc(sizeof(double) * (size_t)B * K::ZDIM * M::EDIM, (cudaStream_t)stream, "cudaMallocAsync(maha scratch)");
@@ -238,6 +263,43 @@ inline void batch_rts(HostCtx<M>& ctx, const double* hx_pred, const double* hP_p
   launch_rts_auto<M>(a, (cudaStream_t)stream);
 }
 
+// ------------------------------------------------------ covariance layout conversion ---
+// Entry e of the compact full-layout buffer `full` [n, EDIM, EDIM] <-> filter idx[e] (e without a list) of the packed
+// batch `packed` [*, packed_doubles(EDIM)].  Packing reads only the lower triangle; unpacking writes its exact mirror.
+template <int E>
+__global__ void __launch_bounds__(256) convert_P_kernel(double* __restrict__ full, double* __restrict__ packed, const int* __restrict__ idx,
+                                                        long long n, int to_packed) {
+  constexpr int PD = packed_doubles(E);
+  const long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (t >= n * (E * E)) return;
+  const long long e = t / (E * E);
+  const int r = (int)(t - e * (E * E)), i = r / E, j = r - i * E;
+  double* pk = packed + (idx ? (long long)idx[e] : e) * PD;
+  if (to_packed) {
+    // every slot of the lower block triangle once, the diagonal blocks' upper slot from its lower mirror
+    if ((i >> 1) >= (j >> 1)) pk[packed_block(i >> 1, j >> 1) + 2 * (i & 1) + (j & 1)] = full[e * (E * E) + (i >= j ? i * E + j : j * E + i)];
+  } else {
+    full[t] = pk[packed_index(i, j)];
+  }
+}
+
+template <class M>
+inline int convert_P(double* full, double* packed, const int* idx, long long n, int to_packed, void* stream) {
+  constexpr int E = M::EDIM;
+  if constexpr (E % 2 == 0 && E <= 32) {
+    if (n <= 0) return 0;
+    const long long threads = n * (E * E);
+    convert_P_kernel<E><<<(unsigned)((threads + 255) / 256), 256, 0, (cudaStream_t)stream>>>(full, packed, idx, n, to_packed);
+    const cudaError_t err = cudaGetLastError();
+    check(err, "convert_P launch");
+    return (int)err;
+  } else {
+    fprintf(stderr, "[rednose_b200] convert_P: no packed covariance layout for EDIM = %d\n", E);
+    last_status() = (int)cudaErrorNotSupported;
+    return (int)cudaErrorNotSupported;
+  }
+}
+
 // --------------------------------------------- batched, HOST buffers (stateless) ---
 // Full round trip: x,P,z,R(,ea) host -> device, fused step, x,P,y device -> host, in
 // chunks on alternating streams so copies overlap the kernel when the host
@@ -249,6 +311,11 @@ inline void host_step(HostCtx<M>& ctx, double* x, double* P, const double* Q, co
                       const int* quat_idxs, int n_quat, int flags) {
   constexpr int D = M::DIM, E = M::EDIM, Z = K::ZDIM, EA = K::EADIM;
   if (!check_quat_idxs(quat_idxs, n_quat, D)) return;   // before any stream, allocation or copy
+  if (flags & FLAG_PACKED_P) {
+    fprintf(stderr, "[rednose_b200] host_step: host buffers hold the full [B, EDIM, EDIM] covariance; FLAG_PACKED_P is not accepted\n");
+    last_status() = (int)cudaErrorNotSupported;
+    return;
+  }
   if (B <= 0) return;
   const long long per = D + E * E + 1 + (long long)n_obs * (Z + Z * Z + EA) + 1;
   constexpr long long PAD = 8;   // each of the six sub-buffers below is rounded up to an even number of doubles

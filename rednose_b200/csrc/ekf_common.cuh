@@ -23,6 +23,7 @@ enum : int {
   FLAG_Q_DIAG             = 4,  // caller promises Q is diagonal (only its diagonal is read)
   FLAG_SHARED_R           = 8,  // R points at ONE [ZDIM, ZDIM] matrix used by every filter / observation
   FLAG_AUGMENT            = 16, // MSCKF: shift the clone window after the (last) update, in the same launch (ekf_sym.py:527-528 -> :365-391); CTA kernel only
+  FLAG_PACKED_P           = 32, // P is [B, packed_doubles(EDIM)] in the packed lower-block-triangle layout (ekf_packed.cuh); pair kernel only
 };
 
 // One argument block per launch, passed by value (lives in the kernel parameter
@@ -30,7 +31,7 @@ enum : int {
 template <int NG>
 struct StepArgs {
   double* x;             // [B, DIM]        in/out
-  double* P;             // [B, EDIM, EDIM] in/out, row-major, symmetric
+  double* P;             // [B, EDIM, EDIM] in/out, row-major, symmetric (lower triangle read); [B, packed_doubles(EDIM)] with FLAG_PACKED_P
   const double* Q;       // [EDIM, EDIM]    batch-shared process noise (ekf_c.c:21,28)
   const double* dt_arr;  // [B] or nullptr -> use dt
   double dt;

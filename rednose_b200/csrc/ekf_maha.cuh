@@ -1,16 +1,24 @@
 // rednose_b200 -- batched Mahalanobis query: d = y^T (H_err P H_err^T + R)^-1 y with y = z - h(x), no state change.
 // Reference: EKF_sym.maha_test, rednose/helpers/ekf_sym.py:626-649 (h, H, H_mod, S^-1 with numpy; no null-space
 // projection even for feature kinds).  A query, not a hot loop: one thread per filter, any EDIM, P read in place
-// through a strided view; the generated sparse KIND::Herr_apply does both H_err P and (H_err P) H_err^T.
+// through a view of its lower triangle (full or packed layout, so both give the same distance); the generated sparse KIND::Herr_apply does both H_err P and (H_err P) H_err^T.
 #pragma once
 #include "ekf_common.cuh"
+#include "ekf_packed.cuh"
 
 namespace rnb {
 
-struct GlobalCol {  // column / row of a row-major matrix in global memory as a vector
-  const double* p;
-  int stride;
-  __device__ __forceinline__ double operator[](int i) const { return __ldg(p + (long long)i * stride); }
+template <int E>
+struct GlobalCol {  // column j of one filter's covariance in global memory as a vector, read from the lower triangle
+  const double* P;  // the filter's covariance: row-major [E, E], or packed (ekf_packed.cuh)
+  int j;
+  bool packed;
+  __device__ __forceinline__ double operator[](int i) const {
+    if constexpr (E % 2 == 0) {
+      if (packed) return __ldg(P + packed_index(i, j));
+    }
+    return __ldg(P + (i >= j ? i * E + j : j * E + i));
+  }
 };
 
 struct ScratchRow {  // written by this very thread earlier in the kernel: plain (coherent) loads, never __ldg
@@ -33,8 +41,10 @@ __global__ void __launch_bounds__(128) ekf_maha_thread(const double* __restrict_
   for (int i = 0; i < Z; ++i) y[i] = z[b * Z + i] - hx[i];
   // HP[c][j] for all columns j -> per-thread scratch (Z x E doubles), then S[:, t] = H_err HP[t, :]^T
   double* hpw = scratch + b * (long long)(Z * E);
+  const bool packed = (E % 2 == 0) && (flags & FLAG_PACKED_P);
+  const double* Pb = P + b * (long long)(packed ? packed_doubles(E) : E * E);
   for (int j = 0; j < E; ++j) {
-    GlobalCol pc{P + b * (long long)(E * E) + j, E};
+    GlobalCol<E> pc{Pb, j, packed};
     double hp[Z];
     K::Herr_apply(hv, pc, hp);
 #pragma unroll

@@ -17,6 +17,7 @@
 // instead of 12) and two independent dependency chains per lane.
 #pragma once
 #include "ekf_warp.cuh"
+#include "ekf_packed.cuh"
 #include <cstdlib>
 
 namespace rnb {
@@ -72,7 +73,7 @@ struct PairScratch {
   alignas(8) uint64_t stg;                            // "staging blocks landed" mbarrier
 };
 
-template <class M, class K, bool PRED, bool UPD, int G, bool GATHER>
+template <class M, class K, bool PRED, bool UPD, int G, bool GATHER, bool PACKED>
 __global__ void __launch_bounds__(32, RNB_PAIR_MIN_WARPS) ekf_step_pair(const StepArgs<M::NG> a) {
   constexpr int D = M::DIM, E = M::EDIM, Z = K::ZDIM;
   using L = RowLayout<M, K>;
@@ -103,7 +104,8 @@ __global__ void __launch_bounds__(32, RNB_PAIR_MIN_WARPS) ekf_step_pair(const St
   double* exh = s.exhp + h * XN;            // this half's exchange / (H P) buffer
 
   constexpr int NST = RNB_STAGES;
-  constexpr uint32_t TILE_BYTES = E * E * sizeof(double);
+  constexpr int TS = PACKED ? packed_doubles(E) : E * E;   // doubles of one filter's covariance in a.P
+  constexpr uint32_t TILE_BYTES = TS * sizeof(double);
   uint32_t it = 0;
   if (lane == 0) {
 #pragma unroll
@@ -119,10 +121,33 @@ __global__ void __launch_bounds__(32, RNB_PAIR_MIN_WARPS) ekf_step_pair(const St
     mbar_expect_tx(&s.full[slot], np * TILE_BYTES);
     double* dst = s.tile + slot * (2 * E * E);
     if constexpr (GATHER) {
-      tma_load_1d(dst, a.P + fidA * (long long)(E * E), TILE_BYTES, &s.full[slot]);
-      if (np == 2) tma_load_1d(dst + E * E, a.P + fidB * (long long)(E * E), TILE_BYTES, &s.full[slot]);
+      tma_load_1d(dst, a.P + fidA * (long long)TS, TILE_BYTES, &s.full[slot]);
+      if (np == 2) tma_load_1d(dst + TS, a.P + fidB * (long long)TS, TILE_BYTES, &s.full[slot]);
     } else {
-      tma_load_1d(dst, a.P + fidA * (long long)(E * E), np * TILE_BYTES, &s.full[slot]);   // consecutive filters: one copy
+      tma_load_1d(dst, a.P + fidA * (long long)TS, np * TILE_BYTES, &s.full[slot]);   // consecutive filters: one copy
+    }
+  };
+  // full row-major a.P (without FLAG_PACKED_P) and hP_filt: the lane writes its lower blocks (I, hl), I >= hl, and their
+  // transposes, so that the stored matrix is the exact mirror of its lower triangle
+  // hP_pred, read only by the RTS backward pass: the lane writes its two columns, one coalesced 128-bit store per row.  Its
+  // lower triangle is what store_full writes, its upper triangle the lane's own values (the mirror up to rounding).  The
+  // transposed stores of store_full hit a different row per lane: on both slabs they made the forward pass with history
+  // 1.5x slower.
+  auto store_cols = [&](double* Pm, const double (&q0)[E], const double (&q1)[E]) {
+#pragma unroll
+    for (int i = 0; i < E; ++i) *reinterpret_cast<double2*>(Pm + i * E + c0) = make_double2(q0[i], q1[i]);
+  };
+  auto store_full = [&](double* Pm, const double (&q0)[E], const double (&q1)[E]) {
+#pragma unroll
+    for (int I = 0; I < E / 2; ++I) {
+      if (I >= hl) {
+        *reinterpret_cast<double2*>(Pm + 2 * I * E + c0) = make_double2(q0[2 * I], I == hl ? q0[2 * I + 1] : q1[2 * I]);
+        *reinterpret_cast<double2*>(Pm + (2 * I + 1) * E + c0) = make_double2(q0[2 * I + 1], q1[2 * I + 1]);
+      }
+      if (I > hl) {
+        *reinterpret_cast<double2*>(Pm + c0 * E + 2 * I) = make_double2(q0[2 * I], q0[2 * I + 1]);
+        *reinterpret_cast<double2*>(Pm + (c0 + 1) * E + 2 * I) = make_double2(q1[2 * I], q1[2 * I + 1]);
+      }
     }
   };
 
@@ -274,17 +299,26 @@ __global__ void __launch_bounds__(32, RNB_PAIR_MIN_WARPS) ekf_step_pair(const St
       const long long b = fid_of(fi);
       double* row = s.rows + fi * RS;
       const uint32_t slot = it % NST;
-      const double* tile = s.tile + slot * (2 * E * E) + (valid ? h : 0) * (E * E);
+      const double* tile = s.tile + slot * (2 * E * E) + (valid ? h : 0) * TS;
       double p0[E], p1[E];                        // columns c0 and c0 + 1
       double fv[L::NFp];
       if (RNB_PAIR_FV_EARLY && do_pred) vec_load(row + L::OFF_FV, fv);
 
       mbar_wait(&s.full[slot], (it / NST) & 1u);
-      // row i of the tile holds P[i][c0], P[i][c0+1] side by side: one 128-bit load per row feeds both columns
+      // P is defined by its lower triangle.  Rows 2I, 2I+1 of the owned columns are the 2x2 block (I, hl) when I >= hl and
+      // the transpose of block (hl, I) when I < hl; either way the block arrives as two 128-bit loads u = first row,
+      // v = second row, and only the two off-diagonal values swap places.  On the diagonal block (I == hl) the upper
+      // element P[c0][c0+1] is taken from its lower mirror v.x.
 #pragma unroll
-      for (int i = 0; i < E; ++i) {
-        const double2 t = *reinterpret_cast<const double2*>(tile + i * E + c0);
-        p0[i] = t.x; p1[i] = t.y;
+      for (int I = 0; I < E / 2; ++I) {
+        const int mx = I > hl ? I : hl, mn = I > hl ? hl : I;
+        const double* pb = tile + (PACKED ? packed_block(mx, mn) : 2 * mx * E + 2 * mn);
+        const double2 u = *reinterpret_cast<const double2*>(pb);
+        const double2 v = *reinterpret_cast<const double2*>(pb + (PACKED ? 2 : E));
+        p0[2 * I] = u.x;
+        p1[2 * I] = I > hl ? u.y : v.x;
+        p0[2 * I + 1] = I >= hl ? v.x : u.y;
+        p1[2 * I + 1] = v.y;
       }
       const int fn = f + 2 * NST;
       const long long fa = fid_of(fn < ng ? fn : 0), fb = fid_of(fn + 1 < ng ? fn + 1 : 0);
@@ -362,11 +396,7 @@ __global__ void __launch_bounds__(32, RNB_PAIR_MIN_WARPS) ekf_step_pair(const St
             p1[i] = fma(dt, __ldg(Qg + i * E + 1), p1[i]);
           }
         }
-        if (a.hP_pred && wr) {
-          double* Hg = a.hP_pred + b * (long long)(E * E) + c0;
-#pragma unroll
-          for (int i = 0; i < E; ++i) *reinterpret_cast<double2*>(Hg + i * E) = make_double2(p0[i], p1[i]);
-        }
+        if (a.hP_pred && wr) store_cols(a.hP_pred + b * (long long)(E * E), p0, p1);
       }
 
       if constexpr (UPD) {
@@ -441,17 +471,24 @@ __global__ void __launch_bounds__(32, RNB_PAIR_MIN_WARPS) ekf_step_pair(const St
           p0[i] = a0; p0[i + 1] = a1; p1[i] = b0v; p1[i + 1] = b1v;
         }
         __syncwarp();
-        if (a.hP_filt && wr && o == n_obs - 1) {
-          double* Hg = a.hP_filt + b * (long long)(E * E) + c0;
-#pragma unroll
-          for (int i = 0; i < E; ++i) *reinterpret_cast<double2*>(Hg + i * E) = make_double2(p0[i], p1[i]);
-        }
+        if (a.hP_filt && wr && o == n_obs - 1) store_full(a.hP_filt + b * (long long)(E * E), p0, p1);   // = the state, bit for bit
       }
 
       if (wr) {
-        double* Pg = a.P + b * (long long)(E * E) + c0;
+        if constexpr (PACKED) {
+          // the lane's blocks (I, hl), I >= hl: one 32-byte block per iteration, two 128-bit stores
+          double* Pg = a.P + b * (long long)TS;
 #pragma unroll
-        for (int i = 0; i < E; ++i) *reinterpret_cast<double2*>(Pg + i * E) = make_double2(p0[i], p1[i]);
+          for (int I = 0; I < E / 2; ++I) {
+            if (I >= hl) {
+              double* q = Pg + packed_block(I, hl);
+              *reinterpret_cast<double2*>(q) = make_double2(p0[2 * I], I == hl ? p0[2 * I + 1] : p1[2 * I]);
+              *reinterpret_cast<double2*>(q + 2) = make_double2(p0[2 * I + 1], p1[2 * I + 1]);
+            }
+          }
+        } else {
+          store_full(a.P + b * (long long)(E * E), p0, p1);
+        }
       }
     }
     __syncwarp();

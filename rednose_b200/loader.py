@@ -2,7 +2,7 @@
 
 ``load_code`` keeps the reference contract: parse ``{folder}/{name}.h`` keeping only the
 lines that start with ``void `` (the only thing cffi's cdef can digest without a
-preprocessor) and ``dlopen`` ``{folder}/lib{name}.so``.  The generated header also carries the
+preprocessor), plus this package's ``int <name>_...`` additions, and ``dlopen`` ``{folder}/lib{name}.so``.  The generated header also carries the
 batched ``<name>_batch_*`` prototypes in the same single-line form, so the very same call
 exposes them.
 """
@@ -31,10 +31,9 @@ def load_code(folder, name):
   lib_path = os.path.join(folder, f"lib{name}.{ext}")
   with open(os.path.join(folder, f"{name}.h"), encoding='utf-8') as f:
     text = f.read()
-  protos = [ln for ln in text.split("\n") if ln.startswith("void ") and not ln.startswith("void* ")]
+  protos = [ln for ln in text.split("\n") if (ln.startswith("void ") and not ln.startswith("void* ")) or ln.startswith(f"int {name}_")]
   ffi = FFI()
-  status_proto = f"int {name}_cuda_status(void);"
-  ffi.cdef("\n".join(protos) + ("\n" + status_proto + "\n" if status_proto in text else "\n"))
+  ffi.cdef("\n".join(protos) + "\n")
   if not os.path.exists(lib_path):
     raise FileNotFoundError(f"{lib_path} is missing: run the filter's generator (gen_code) first")
   return ffi, ffi.dlopen(lib_path)

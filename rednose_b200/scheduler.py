@@ -88,7 +88,7 @@ class RewindingScheduler(RaggedScheduler):
     f64 = dict(dtype=torch.float64, device=dev)
     self.ring_t = torch.full((B, self.N), float("nan"), **f64)
     self.ring_x = torch.zeros(B, self.N, engine.x.shape[1], **f64)
-    E = engine.P.shape[1]
+    E = self.E = engine.dim_err if hasattr(engine, "dim_err") else engine.P.shape[1]
     self.packed = bool(packed)
     if self.packed:
       tr = torch.tril_indices(E, E, device=dev)
@@ -109,6 +109,17 @@ class RewindingScheduler(RaggedScheduler):
     self.replayed = 0                                            # observations re-applied during fast-forward
 
   # -- ring -----------------------------------------------------------------------------------------------------------
+  # rows of P through the engine's row accessors when it has them (BatchedEKF: touches only those filters of its
+  # resident covariance), else by indexing a plain P tensor
+  def _get_P(self, ids):
+    return self.e.get_P_rows(ids) if hasattr(self.e, "get_P_rows") else self.e.P[ids]
+
+  def _set_P(self, ids, P):
+    if hasattr(self.e, "set_P_rows"):
+      self.e.set_P_rows(ids, P)
+    else:
+      self.e.P[ids] = P
+
   def _push(self, ids, t, kind, z, R, ea):
     """Checkpoint the CURRENT state of filters `ids` together with the observation just applied (ekf_sym.py:437-450)."""
     full = self.cnt[ids] == self.N
@@ -116,7 +127,8 @@ class RewindingScheduler(RaggedScheduler):
     m = z.shape[-1]
     self.ring_t[ids, pos] = t
     self.ring_x[ids, pos] = self.e.x[ids]
-    self.ring_P[ids, pos] = self.e.P[ids][:, self._tri_r, self._tri_c] if self.packed else self.e.P[ids]
+    P = self._get_P(ids)
+    self.ring_P[ids, pos] = P[:, self._tri_r, self._tri_c] if self.packed else P
     self.ring_kind[ids, pos] = kind
     self.ring_z[ids, pos, :m] = z
     self.ring_R[ids, pos, :m, :m] = R
@@ -192,10 +204,10 @@ class RewindingScheduler(RaggedScheduler):
         src = phys.gather(1, (idx - 1)[:, None])[:, 0]
         self.e.x[lf] = self.ring_x[lf, src]                              # ekf_sym.py:425-427
         if self.packed:
-          E = self.e.P.shape[1]
-          self.e.P[lf] = self.ring_P[lf, src][:, self._unpack].reshape(-1, E, E)
+          E = self.E
+          self._set_P(lf, self.ring_P[lf, src][:, self._unpack].reshape(-1, E, E))
         else:
-          self.e.P[lf] = self.ring_P[lf, src]
+          self._set_P(lf, self.ring_P[lf, src])
         self.t_filter[lf] = self.ring_t[lf, src]
         # the observations rewound over (logical idx .. cnt-1), copied out before the ring is reused
         n_rep = cnt - idx
