@@ -53,7 +53,9 @@ __global__ void __launch_bounds__(RTS_WARPS * 32, RTS_MIN_CTAS) ekf_rts_warp_mma
   using SC = RtsMmaScratch<M>;
   constexpr int LD = SC::LD, NP = SC::NP, LP = SC::LP, NT = NP / 8, NK = NP / 4;
   static_assert(E <= 32 && E % 2 == 0, "fragment I/O needs an even EDIM <= 32");
-  __shared__ SC s_all[RTS_WARPS];
+  // dynamic: from a main block of 25 (NP = 32) the RTS_WARPS scratch blocks pass the 48 KB static limit
+  extern __shared__ __align__(16) unsigned char rts_smem_raw[];
+  SC* s_all = reinterpret_cast<SC*>(rts_smem_raw);
   const int lane = threadIdx.x & 31, wib = threadIdx.x >> 5;
   const long long b = (long long)blockIdx.x * RTS_WARPS + wib;
   if (b >= a.B) return;
@@ -302,7 +304,10 @@ inline void launch_rts_auto(const RtsArgs<M::NG>& a, cudaStream_t st) {
   if (a.B <= 0 || a.T <= 0) return;
   if constexpr (RNB_RTS_MMA && M::EDIM <= 32 && M::EDIM % 2 == 0 && M::MEDIM >= 8) {
     const unsigned grid = (unsigned)((a.B + RTS_WARPS - 1) / RTS_WARPS);
-    ekf_rts_warp_mma<M><<<grid, RTS_WARPS * 32, 0, st>>>(a);
+    constexpr size_t smem = sizeof(RtsMmaScratch<M>) * RTS_WARPS;   // 55 296 B at EDIM 32, 32 192 B for live_kf
+    if (first_launch_of((const void*)ekf_rts_warp_mma<M>))
+      cudaFuncSetAttribute(ekf_rts_warp_mma<M>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    ekf_rts_warp_mma<M><<<grid, RTS_WARPS * 32, smem, st>>>(a);
     check(cudaGetLastError(), "ekf_rts_mma launch");
   } else {
     launch_rts<M>(a, st);
