@@ -134,7 +134,8 @@ inline void launch_step(const StepArgs<M::NG>& a, cudaStream_t st) {
         return;
       }
       constexpr int G = RNB_PAIR_GROUP;
-      constexpr size_t smem = pair_smem_bytes<M, K, G>();
+      const bool packed = a.flags & FLAG_PACKED_P;
+      const size_t smem = packed ? pair_smem_bytes<M, K, G, true>() : pair_smem_bytes<M, K, G, false>();
       const unsigned grid = (unsigned)((a.B + G - 1) / G);
       auto run = [&](void (*kern)(const StepArgs<M::NG>)) {
         if (first_launch_of((const void*)kern)) {
@@ -143,7 +144,6 @@ inline void launch_step(const StepArgs<M::NG>& a, cudaStream_t st) {
         }
         kern<<<grid, 32, smem, st>>>(a);
       };
-      const bool packed = a.flags & FLAG_PACKED_P;
       if constexpr (PRED && UPD) {
         if (a.idx) run(packed ? ekf_step_pair<M, K, PRED, UPD, G, true, true> : ekf_step_pair<M, K, PRED, UPD, G, true, false>);
         else run(packed ? ekf_step_pair<M, K, PRED, UPD, G, false, true> : ekf_step_pair<M, K, PRED, UPD, G, false, false>);

@@ -44,12 +44,19 @@ namespace rnb {
 #define RNB_PAIR_TMA_STAGE 1   // x / z / R / dt blocks of a full group arrive by bulk copy (one mbarrier wait, no registers held)
 #endif
 
-template <class M, class K, int G>
+// Depth of the covariance tile ring (pairs in flight per warp).  A packed pair (live_kf: 4 224 B) is little more than half
+// a full one (7 744 B), so with the packed layout two slots cost about what one full slot does and the warp keeps two
+// pairs in flight at 8 warps per SM; the full layout (unflagged ABI, host_step) keeps RNB_STAGES slots of its size.
+template <bool PACKED>
+constexpr int pair_stages() { return PACKED ? 2 : RNB_STAGES; }
+
+template <class M, class K, int G, bool PACKED>
 struct PairScratch {
   using L = RowLayout<M, K>;
   static constexpr int E = M::EDIM;
-  static constexpr int NST = RNB_STAGES;
-  alignas(128) double tile[NST * 2 * E * E];          // covariance tile PAIRS (TMA ring)
+  static constexpr int NST = pair_stages<PACKED>();
+  static constexpr int TS = PACKED ? packed_doubles(E) : E * E;   // doubles of one filter's covariance tile
+  alignas(128) double tile[NST * 2 * TS];             // covariance tile PAIRS (TMA ring)
   alignas(8) uint64_t full[NST];
   alignas(16) double rows[G * L::STRIDE];
   static constexpr int EXS = ((E + 3) & ~3) + 2;      // exchange row stride, = 2 (mod 4): see WarpScratch
@@ -77,7 +84,7 @@ template <class M, class K, bool PRED, bool UPD, int G, bool GATHER, bool PACKED
 __global__ void __launch_bounds__(32, RNB_PAIR_MIN_WARPS) ekf_step_pair(const StepArgs<M::NG> a) {
   constexpr int D = M::DIM, E = M::EDIM, Z = K::ZDIM;
   using L = RowLayout<M, K>;
-  using SC = PairScratch<M, K, G>;
+  using SC = PairScratch<M, K, G, PACKED>;
   constexpr int RS = L::STRIDE, HPS = SC::HPS, XN = SC::XN;
   static_assert(E <= 32 && E % 2 == 0, "pair kernel: even EDIM <= 32");
   static_assert(G <= 32 && G % 2 == 0, "group size");
@@ -103,8 +110,8 @@ __global__ void __launch_bounds__(32, RNB_PAIR_MIN_WARPS) ekf_step_pair(const St
   };
   double* exh = s.exhp + h * XN;            // this half's exchange / (H P) buffer
 
-  constexpr int NST = RNB_STAGES;
-  constexpr int TS = PACKED ? packed_doubles(E) : E * E;   // doubles of one filter's covariance in a.P
+  constexpr int NST = SC::NST;
+  constexpr int TS = SC::TS;                // doubles of one filter's covariance in a.P
   constexpr uint32_t TILE_BYTES = TS * sizeof(double);
   uint32_t it = 0;
   if (lane == 0) {
@@ -119,7 +126,7 @@ __global__ void __launch_bounds__(32, RNB_PAIR_MIN_WARPS) ekf_step_pair(const St
   auto issue_pair = [&](int f, uint32_t slot, long long fidA, long long fidB) {
     const int np = (ng - f >= 2) ? 2 : 1;
     mbar_expect_tx(&s.full[slot], np * TILE_BYTES);
-    double* dst = s.tile + slot * (2 * E * E);
+    double* dst = s.tile + slot * (2 * TS);
     if constexpr (GATHER) {
       tma_load_1d(dst, a.P + fidA * (long long)TS, TILE_BYTES, &s.full[slot]);
       if (np == 2) tma_load_1d(dst + TS, a.P + fidB * (long long)TS, TILE_BYTES, &s.full[slot]);
@@ -299,7 +306,7 @@ __global__ void __launch_bounds__(32, RNB_PAIR_MIN_WARPS) ekf_step_pair(const St
       const long long b = fid_of(fi);
       double* row = s.rows + fi * RS;
       const uint32_t slot = it % NST;
-      const double* tile = s.tile + slot * (2 * E * E) + (valid ? h : 0) * TS;
+      const double* tile = s.tile + slot * (2 * TS) + (valid ? h : 0) * TS;
       double p0[E], p1[E];                        // columns c0 and c0 + 1
       double fv[L::NFp];
       if (RNB_PAIR_FV_EARLY && do_pred) vec_load(row + L::OFF_FV, fv);
@@ -518,8 +525,8 @@ __global__ void __launch_bounds__(32, RNB_PAIR_MIN_WARPS) ekf_step_pair(const St
   }
 }
 
-template <class M, class K, int G>
-constexpr size_t pair_smem_bytes() { return sizeof(PairScratch<M, K, G>); }
+template <class M, class K, int G, bool PACKED>
+constexpr size_t pair_smem_bytes() { return sizeof(PairScratch<M, K, G, PACKED>); }
 
 template <class M>
 constexpr bool use_pair() { return RNB_PAIR && RNB_TMA && M::EDIM % 2 == 0 && M::EDIM <= 32; }
