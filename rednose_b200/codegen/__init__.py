@@ -34,6 +34,17 @@ def _matsym_name(m):
   return str(m.name) if hasattr(m, 'name') else str(m)
 
 
+# dynamic shared memory one CTA may opt in to on sm_90 (227 KB)
+MAX_SMEM_PER_BLOCK = 232448
+
+
+def augment_smem_bytes(edim, dim):
+  """Dynamic shared memory of ekf_augment_cta (csrc/ekf_augment.cuh): the whole covariance and state of one filter.
+  It bounds an MSCKF's size: ekf_step_cta keeps only the lower triangle plus a ZDIM-wide panel (ZDIM <= 31 + EADIM), which
+  is the larger of the two only below EDIM ~120, where both need less than half the limit."""
+  return 8 * (edim * edim + dim)
+
+
 def _fma_chain(terms, init=None):
   """terms: [(coef_c, var_c)] -> nested fma expression string."""
   acc = init
@@ -79,6 +90,11 @@ def gen_code(folder, name, f_sym, dt_sym, x_sym, obs_eqs, dim_x, dim_err, eskf_p
     raise ValueError(f"filter '{name}': main error block of {int(dim_main_err)} states; the kernels serve at most 32 (the "
                      f"rows of F that differ from the identity are one 32-bit mask).  A larger state needs an MSCKF layout "
                      f"(msckf_params) whose main block is at most 32.")
+  if msckf and augment_smem_bytes(int(dim_err), int(dim_x)) > MAX_SMEM_PER_BLOCK:
+    raise ValueError(f"filter '{name}': EDIM {int(dim_err)}, DIM {int(dim_x)}: the clone-window shift (ekf_augment_cta) "
+                     f"stages the whole covariance and state of a filter in shared memory, "
+                     f"{augment_smem_bytes(int(dim_err), int(dim_x))} bytes, over the {MAX_SMEM_PER_BLOCK} bytes one CTA "
+                     f"can have.  Use fewer or smaller clones.")
 
   f_sym = sp.Matrix(f_sym)
   H_mod_sym = sp.Matrix(H_mod_sym)
@@ -121,6 +137,7 @@ def gen_code(folder, name, f_sym, dt_sym, x_sym, obs_eqs, dim_x, dim_err, eskf_p
   out.append(f"struct {model} {{\n")
   out.append(f"  static constexpr int DIM = {DIM}, EDIM = {EDIM}, MEDIM = {MEDIM}, DMAIN = {int(dim_main)}, NG = {NG};\n")
   out.append(f"  static constexpr int DAUG = {int(dim_augment) if msckf else 0}, EAUG = {int(dim_augment_err) if msckf else 0};   // clone size (state / error state), ekf_sym.py:57-66\n")
+  out.append(f"  static constexpr bool HAS_FEATURE_KIND = {'true' if any(kd['feature'] for kd in kinds) else 'false'};   // a feature kind runs on the CTA kernel: P stays in the full layout\n")
 
   # f_fun, F_dense, H_mod_dense, err_fun, inv_err_fun: reference-shaped leaf functions
   pr = printer({xname: 'state'})

@@ -83,10 +83,12 @@ struct HostCtx {
 constexpr int THREAD_MAX_EDIM = 6;
 
 // true when a step of filter M serves its covariance with the pair kernel (ekf_warp2.cuh), the only kernel that reads
-// and writes the packed layout; reads REDNOSE_B200_WARP_KERNEL at call time, like launch_step
+// and writes the packed layout; reads REDNOSE_B200_WARP_KERNEL at call time, like launch_step.  A filter with a
+// feature-track kind is never served whole by the pair kernel (its feature kinds run on the CTA kernel, which reads the
+// full layout), so its P stays full
 template <class M>
 inline bool pair_serves() {
-  if constexpr (M::EDIM > THREAD_MAX_EDIM && use_pair<M>()) return pair_enabled();
+  if constexpr (M::EDIM > THREAD_MAX_EDIM && use_pair<M>() && !M::HAS_FEATURE_KIND) return pair_enabled();
   else return false;
 }
 

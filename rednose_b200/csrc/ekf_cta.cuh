@@ -337,20 +337,21 @@ __global__ void __launch_bounds__(cta_threads<M>(), RNB_CTA_MIN_BLOCKS) ekf_step
       for (int c = 0; c < Z; ++c) s.U[col * HL + c] = hp[c];  // unprojected, for S
     }
     __syncthreads();
-    // S_raw[:, t] = H_err (HP_raw[t, :])^T   (P symmetric)
-    if (tid < Z) {
-      SmemCol<Z> hr{&s.U[tid], HL};
+    // S_raw[:, t] = H_err (HP_raw[t, :])^T   (P symmetric); a one-warp CTA has fewer threads than a ZDIM of 33-34
+    for (int t = tid; t < Z; t += nth) {
+      SmemCol<Z> hr{&s.U[t], HL};
       double sc[Z];
       K::Herr_apply(s.hv, hr, sc);
 #pragma unroll
-      for (int c = 0; c < Z; ++c) s.S[c * SL + tid] = sc[c];
+      for (int c = 0; c < Z; ++c) s.S[c * SL + t] = sc[c];
     }
     __syncthreads();
     if constexpr (K::HAS_HE) {
-      // project S and R on both sides, y and HP on the left; S and R are handled by two different warps
-      const int w = warp, t = lane;
+      // project S and R on both sides, y and HP on the left; S and R are handled by two different warps, each lane
+      // taking columns (rows) lane, lane + 32 (ZDIM may exceed 32 by up to EADIM - 1: Y + 1 <= 32)
+      const int w = warp;
       for (int mx = w; mx < 2; mx += nw) {
-        if (t < Z) {  // columns
+        for (int t = lane; t < Z; t += 32) {  // columns
           double* Mx = (mx == 0) ? s.S : s.Rm;
           double u[Z];
 #pragma unroll
@@ -363,7 +364,7 @@ __global__ void __launch_bounds__(cta_threads<M>(), RNB_CTA_MIN_BLOCKS) ekf_step
       if (own) apply_reflectors<Z, NR>(s.V, s.beta, hp);
       __syncthreads();
       for (int mx = w; mx < 2; mx += nw) {
-        if (t < Z) {  // rows
+        for (int t = lane; t < Z; t += 32) {  // rows
           double* Mx = (mx == 0) ? s.S : s.Rm;
           double u[Z];
 #pragma unroll

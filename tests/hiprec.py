@@ -9,9 +9,11 @@ them (for a plain EKF: identity injection and H_mod = I), so nothing is rounded 
 and the result.  The result is therefore the exact answer to rounding at 1e-40, against which float64 implementations
 (the CUDA kernels, the CPU oracle) can each be measured.
 
-Any model gen_code accepts without an MSCKF layout works: ESKF or plain, observation kinds with extra arguments, global
-variables (``HiPrecModel.gv``).  The batch helpers (``step``, ``predict``, ``update``, ``maha``, ``rts``) take float64
-arrays over filters and return float64 arrays.
+Any model gen_code accepts works: ESKF or plain, observation kinds with extra arguments, global variables
+(``HiPrecModel.gv``), and the MSCKF layout (``msckf_params``): a feature-track kind is projected on an orthonormal basis
+of the left null space of He = dh/d(ea), computed at 40 digits, and ``augment`` is the clone-window shift.  x and P do not
+depend on the basis; the projected innovation does, so only its norm can be compared.  The batch helpers (``step``,
+``predict``, ``update``, ``maha``, ``augment``, ``rts``) take float64 arrays over filters and return float64 arrays.
 
 Pure Python: a 22x22 product costs about 10 ms, so keep it to a few filters and a few dozen steps.
 It needs neither the reference checkout nor any compiled library.
@@ -44,8 +46,12 @@ def model_of(filter_cls):
 class HiPrecModel:
   """Leaf functions of one model (the arguments gen_code receives), evaluated in mpmath."""
 
-  def __init__(self, f_sym, dt_sym, x_sym, obs_eqs, dim_x, dim_err, eskf_params=None, maha_test_kinds=(), global_vars=None, **_):
+  def __init__(self, f_sym, dt_sym, x_sym, obs_eqs, dim_x, dim_err, eskf_params=None, maha_test_kinds=(), global_vars=None,
+               msckf_params=None, **_):
     self.dim_x, self.dim_err = int(dim_x), int(dim_err)
+    # MSCKF layout (ekf_sym.py:57-73): (DIM_MAIN, DAUG, MEDIM, EAUG, N, feature-track kinds)
+    self.msckf = [int(v) for v in msckf_params[:5]] if msckf_params else None
+    self.feature_kinds = set(int(k) for k in msckf_params[5]) if msckf_params else set()
     if eskf_params:
       inject, invert, H_mod_sym, f_err_sym, x_err_sym = eskf_params[:5]
       err = sp.Matrix(x_err_sym)
@@ -70,6 +76,8 @@ class HiPrecModel:
       args = [x_sym] + ([ea_sym] if ea_sym is not None else []) + g
       self._sym[('h', int(kind))] = (args, h_sym)
       self._sym[('H', int(kind))] = (args, h_sym.jacobian(sp.Matrix(x_sym)))
+      if int(kind) in self.feature_kinds:
+        self._sym[('He', int(kind))] = (args, h_sym.jacobian(sp.Matrix(ea_sym)))
       self.zdim[int(kind)] = int(h_sym.shape[0])
       self.eadim[int(kind)] = int(ea_sym.shape[0]) if ea_sym is not None else 0
     self.maha_test_kinds = set(int(k) for k in maha_test_kinds)
@@ -105,6 +113,10 @@ class HiPrecModel:
   def H(self, kind, x, ea=None):
     return _reshape(self._fn(('H', kind))(x, *([ea] if ea is not None else []), *self._g()), self.zdim[kind], self.dim_x)
 
+  def He(self, kind, x, ea):
+    """d h / d ea of a feature-track kind (ZDIM x EADIM)."""
+    return _reshape(self._fn(('He', kind))(x, ea, *self._g()), self.zdim[kind], self.eadim[kind])
+
   def err_fun(self, nom, delta):
     return mp.matrix(self._fn('err')(nom, delta, *self._g()))
 
@@ -114,18 +126,31 @@ class HiPrecModel:
   # ---- one filter ----
   def predict(self, x, P, Q, dt):
     F = self.F(x, dt)
-    return self.f(x, dt), _mul(_mul(F, P), F.T) + dt * Q
+    # F (F P)^T, transposed: the sparse F is the left operand of both products (an MSCKF's F is the identity on the
+    # clones, so this costs ~nnz(F) E instead of E^3 products)
+    return self.f(x, dt), _mul(F, _mul(F, P).T).T + dt * Q
 
   def maha(self, kind, x, P, z, R, ea=None):
-    """y^T S^-1 y of one observation (no state change)."""
+    """y^T S^-1 y of one observation (no state change; a feature kind is not projected, ekf_sym.py:626-649)."""
     y = z - self.h(kind, x, ea)
     He = _mul(self.H(kind, x, ea), self.H_mod(x))
     return (y.T * mp.inverse(_mul(He, P) * He.T + R) * y)[0, 0]
 
+  def null_basis(self, kind, x, ea):
+    """An orthonormal basis A (ZDIM x (ZDIM - EADIM)) of the left null space of He = dh/d(ea): the trailing columns of
+    the full QR factor of He at 40 digits."""
+    Qf, _ = mp.qr(self.He(kind, x, ea), mode='full')
+    Z, EA = self.zdim[kind], self.eadim[kind]
+    return Qf[:, EA:Z] if Z - EA > 1 else mp.matrix([[Qf[i, EA]] for i in range(Z)])
+
   def update(self, kind, x, P, z, R, ea=None, maha_thresh=None):
-    """Returns (x, P, y).  maha_thresh: the gate of a Mahalanobis-tested kind (None: no gate)."""
+    """Returns (x, P, y).  maha_thresh: the gate of a Mahalanobis-tested kind (None: no gate).  A feature-track kind is
+    projected on the left null space of He (ekf_c.c:66-85): y' = A^T y, H' = A^T H_err, R' = A^T R A, and y is y'."""
     y = z - self.h(kind, x, ea)
     He = _mul(self.H(kind, x, ea), self.H_mod(x))
+    if kind in self.feature_kinds:
+      A = self.null_basis(kind, x, ea)
+      y, He, R = A.T * y, _mul(A.T, He), A.T * R * A
     HP = _mul(He, P)
     S = HP * He.T + R
     if maha_thresh is not None and (y.T * mp.inverse(S) * y)[0, 0] > maha_thresh:
@@ -136,6 +161,21 @@ class HiPrecModel:
     # at 40 digits the two differ by ~1e-38 x cond(S), far below float64; it costs E Z E instead of 2 E^3 products
     P = P - K * HP
     return self.err_fun(x, K * y), P, y
+
+  def augment(self, x, P):
+    """The MSCKF clone-window shift (ekf_sym.py:365-391): drop the oldest clone, append a copy of the first DAUG main
+    states; the same selection on the rows and columns of P (the reference's selection-matrix products, whose every
+    entry is one product by 1)."""
+    d1, d3, d2, d4, _ = self.msckf
+    D, E = self.dim_x, self.dim_err
+    sx = list(range(d1)) + list(range(d1 + d3, D)) + list(range(d3))
+    se = list(range(d2)) + list(range(d2 + d4, E)) + list(range(d4))
+    xo = mp.matrix([x[i] for i in sx])
+    Po = mp.matrix(E, E)
+    for i in range(E):
+      for j in range(E):
+        Po[i, j] = P[se[i], se[j]]
+    return xo, Po
 
   @staticmethod
   def normalize(x, quat_idxs):
@@ -198,6 +238,10 @@ class HiPrecModel:
     ea_args = [ea] if ea is not None else []
     He = self.np_leaf(('H', kind), x, *ea_args).reshape(self.zdim[kind], D) @ self.np_leaf('H_mod', x).reshape(D, E)
     y = z - self.np_leaf(('h', kind), x, *ea_args)
+    if kind in self.feature_kinds:            # left-null-space projection with numpy's own (complete) QR basis
+      Hea = self.np_leaf(('He', kind), x, ea).reshape(self.zdim[kind], self.eadim[kind])
+      A = np.linalg.qr(Hea, mode='complete')[0][:, self.eadim[kind]:]
+      y, He, R = A.T @ y, A.T @ He, A.T @ R @ A
     S = He @ P @ He.T + R
     K = np.linalg.solve(S, He @ P.T).T
     IKH = np.eye(E) - K @ He
@@ -332,6 +376,16 @@ def maha(m, kind, x, P, z, R, ea=None, sel=None):
       _, zl, Rl, el = _per_obs(z, R, ea, b)
       out.append(float(m.maha(kind, to_mp(x[b]), to_mp(P[b]), zl[0], Rl[0], el[0])))
   return np.array(out)
+
+
+def augment(m, x, P, sel=None):
+  """The clone-window shift of the filters `sel` of a float64 batch; returns float64 (x, P)."""
+  sel = range(x.shape[0]) if sel is None else sel
+  xs, Ps = [], []
+  for b in sel:
+    xb, Pb = m.augment(to_mp(x[b]), to_mp(P[b]))
+    xs.append(to_np(xb)); Ps.append(to_np(Pb, matrix=True))
+  return np.stack(xs), np.stack(Ps)
 
 
 def rts(m, x_pred, x_filt, P_pred, P_filt, t, quat_idxs=(), norm_quats=False, sel=None):
