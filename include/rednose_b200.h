@@ -16,6 +16,11 @@
  *   batched additions, DEVICE pointers, B independent filters, AoS row-major float64
  *     void <name>_batch_predict(...), <name>_batch_update_<kind>(...), <name>_batch_step_<kind>(...)
  *     void <name>_batch_rts(...)   RTS smoother over a time-major history [T, B, ...]  (ekf_sym.py:651-690)
+ *   ragged histories (every filter records and smooths its own steps; int results = the call's cudaError_t):
+ *     int <name>_batch_step_<kind>_hist_idx(...)   the gather step of <name>_batch_step_<kind>_idx; entry e also records at
+ *         row hist_row[e] (negative: not recorded) of [T, hist_B, ...] history slabs
+ *     int <name>_batch_rts_ragged(...)   filter b smooths rows 0 .. len[b] - 1 with its times t [T, B]; rows >= len[b]
+ *         of xs / Ps are left as they are.  EDIM <= 32 only (cudaErrorNotSupported otherwise)
  *   batched, HOST pointers (copies inside): <name>_host_step_<kind>(...)
  *   packed covariance layout (int results, so the reference's `void ` prototype set is unchanged):
  *     int <name>_packed_P_doubles(void)   doubles per filter of the packed layout, 0 where it is not used
@@ -56,6 +61,10 @@ typedef void (*rednose_batch_step_fn)(double *x, double *P, const double *Q, con
 typedef void (*rednose_host_step_fn)(double *x, double *P, const double *Q, const double *dt_arr, double dt, double *z, const double *R, const double *ea, int n_obs, long long B, const int *quat_idxs, int n_quat, int flags);
 
 typedef void (*rednose_batch_rts_fn)(const double *hx_pred, const double *hP_pred, const double *hx_filt, const double *hP_filt, const double *t, int t_per_filter, double *xs, double *Ps, int T, long long B, const int *quat_idxs, int n_quat, int norm_quats, void *stream);
+/* ragged histories: records entry e at row hist_row[e] (negative: not recorded) of slabs with filter stride hist_B */
+typedef int (*rednose_batch_step_hist_idx_fn)(double *x, double *P, const double *Q, const double *dt_arr, double dt, double *z, const double *R, const double *ea, int n_obs, long long B, const int *quat_idxs, int n_quat, int flags, double *hx_pred, double *hP_pred, double *hx_filt, double *hP_filt, const int *idx, const int *hist_row, long long hist_B, void *stream);
+/* ragged histories: filter b smooths its first len[b] of T rows, times t [T, B] */
+typedef int (*rednose_batch_rts_ragged_fn)(const double *hx_pred, const double *hP_pred, const double *hx_filt, const double *hP_filt, const double *t, const int *len, double *xs, double *Ps, int T, long long B, const int *quat_idxs, int n_quat, int norm_quats, void *stream);
 
 /* Plugin descriptor: replaces `struct EKF` (ekf.h:16-33).  Arrays have n_kinds entries,
  * parallel to `kinds`. */

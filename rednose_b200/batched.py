@@ -204,10 +204,13 @@ class BatchedEKF:
     self._check(f"batch_update_{kind}")
     return z
 
-  def step_indexed(self, kind, idx, dt, z, R, ea=None):
+  def step_indexed(self, kind, idx, dt, z, R, ea=None, hist=None, t=None):
     """Fused predict + update of `kind` for the filters listed in `idx` only ([n] int32, device): entry e uses
     z[e], R[e] (or one shared R), dt[e] and works on filter idx[e].  Filters not listed are untouched.  This is the
-    building block of the ragged scheduler (per-tick kind buckets)."""
+    building block of the ragged scheduler (per-tick kind buckets).
+
+    With a RaggedHistory `hist`, entry e also records its step at filter idx[e]'s next row, with time t[e] (scalar
+    or [n]); a filter whose T rows are used up still steps and counts an overflow."""
     idx = idx.to(device=self.device, dtype=torch.int32).contiguous()
     n = int(idx.shape[0])
     if n == 0:
@@ -230,11 +233,22 @@ class BatchedEKF:
     else:
       dt_ptr, dt_s = self._ffi.NULL, float(dt)
     P, pflag = self._P_arg()
+    idx_p = self._ffi.cast("const int *", idx.data_ptr())
     with torch.cuda.device(self.device):
-      getattr(self._lib, f"{self.name}_batch_step_{kind}_idx")(
-        self._p(self.x), P, self._cp(self.Q), dt_ptr, dt_s, self._p(z), self._cp(R), self._cp(ea),
-        z.shape[1], n, self._quat, self._nquat, flags | pflag, self._ffi.NULL, self._ffi.NULL, self._ffi.NULL, self._ffi.NULL,
-        self._ffi.cast("const int *", idx.data_ptr()), self._stream())
+      if hist is None:
+        getattr(self._lib, f"{self.name}_batch_step_{kind}_idx")(
+          self._p(self.x), P, self._cp(self.Q), dt_ptr, dt_s, self._p(z), self._cp(R), self._cp(ea),
+          z.shape[1], n, self._quat, self._nquat, flags | pflag, self._ffi.NULL, self._ffi.NULL, self._ffi.NULL, self._ffi.NULL,
+          idx_p, self._stream())
+      else:
+        assert t is not None, "a recorded step needs its time"
+        assert hist.B == self.B, (hist.B, self.B)
+        rows = hist.reserve(idx, t)
+        getattr(self._lib, f"{self.name}_batch_step_{kind}_hist_idx")(
+          self._p(self.x), P, self._cp(self.Q), dt_ptr, dt_s, self._p(z), self._cp(R), self._cp(ea),
+          z.shape[1], n, self._quat, self._nquat, flags | pflag,
+          self._p(hist.x_pred), self._p(hist.P_pred), self._p(hist.x_filt), self._p(hist.P_filt),
+          idx_p, self._ffi.cast("const int *", rows.data_ptr()), hist.B, self._stream())
     self.launches += 1
     self._check(f"batch_step_{kind}_idx")
     return z
@@ -353,6 +367,11 @@ class BatchedEKF:
     9-tuples returned by predict_and_update_batch (ekf_sym.py:531): x_{k|k-1}, x_{k|k}, P_{k|k-1}, P_{k|k}, t."""
     return History(T, self.B, self.dim_x, self.dim_err, self.device)
 
+  def new_ragged_history(self, T):
+    """Device slabs for up to T recorded steps PER FILTER, each filter on its own clock (step_indexed(..., hist=)):
+    row k of filter b is the k-th step that filter recorded."""
+    return RaggedHistory(T, self.B, self.dim_x, self.dim_err, self.device)
+
   def step_recorded(self, hist, kind, t, z, R, ea=None):
     """predict_and_update_batch that also appends this step to `hist` (the kernel writes the slabs itself)."""
     k = hist.n
@@ -375,7 +394,13 @@ class BatchedEKF:
     `terminal=(x [B, DIM], P [B, EDIM, EDIM])` smooths one SEGMENT of a longer history (steps k0 .. k0 + T - 2): the
     recursion starts from that smoothed estimate of step k0 + T - 1, whose history entry (the last one recorded) only
     contributes its predicted state; its row of xs / Ps is not written.
+
+    With a RaggedHistory every filter is smoothed over its own n[b] rows and times, and (xs, Ps) are [T, B, ...]: row k
+    of filter b is the smoothed estimate of its k-th recorded step; rows >= n[b] are not written (NaN in a new buffer).
+    Raises if a filter outran the history.
     """
+    if isinstance(hist, RaggedHistory):
+      return self._rts_smooth_ragged(hist, norm_quats, quaternion_idxs, in_place, out, terminal, k0)
     T = hist.n
     assert T >= 1
     hist.sync_times()
@@ -400,6 +425,31 @@ class BatchedEKF:
     self.launches += 1
     self._check("batch_rts")
     return xs[:T], Ps[:T]
+
+  def _rts_smooth_ragged(self, hist, norm_quats, quaternion_idxs, in_place, out, terminal, k0):
+    if terminal is not None or k0:
+      raise ValueError("a ragged history is smoothed whole: segment continuation (terminal, k0) does not apply")
+    lost = hist.overflowed()
+    if lost:
+      raise RuntimeError(f"ragged history overflow: {lost} step(s) found their filter's {hist.T} rows used up and were "
+                         f"not recorded; record into a longer history")
+    if out is not None:
+      xs, Ps = out
+      assert xs.shape == hist.x_filt.shape and Ps.shape == hist.P_filt.shape and xs.is_contiguous() and Ps.is_contiguous()
+    elif in_place:
+      xs, Ps = hist.x_filt, hist.P_filt
+    else:
+      xs = torch.full_like(hist.x_filt, float("nan"))
+      Ps = torch.full_like(hist.P_filt, float("nan"))
+    qi = self._ffi.new("int[]", list(quaternion_idxs) or [0])
+    with torch.cuda.device(self.device):
+      getattr(self._lib, f"{self.name}_batch_rts_ragged")(
+        self._cp(hist.x_pred), self._cp(hist.P_pred), self._cp(hist.x_filt), self._cp(hist.P_filt), self._cp(hist.t),
+        self._ffi.cast("const int *", hist.n.data_ptr()), self._p(xs), self._p(Ps), hist.T, self.B, qi,
+        len(quaternion_idxs) if norm_quats else 0, 1 if norm_quats else 0, self._stream())
+    self.launches += 1
+    self._check("batch_rts_ragged")
+    return xs, Ps
 
 
 class _PackedGraph:
@@ -438,3 +488,45 @@ class History:
 
   def bytes(self):
     return sum(t.numel() * 8 for t in (self.x_pred, self.x_filt, self.P_pred, self.P_filt, self.t))
+
+
+class RaggedHistory:
+  """Per-filter histories of a batch whose filters step on their own clocks (BatchedEKF.step_indexed with hist=).
+
+  Slabs are [T, B, ...] in the full covariance layout, like History, but row k of filter b is the k-th step THAT
+  filter recorded: `n [B]` (int32) counts the rows each filter has used and `t [T, B]` holds their times.  A step of a
+  filter whose T rows are used up is not recorded; `overflow` counts those steps.  All bookkeeping stays on the
+  device (no host synchronisation per tick)."""
+
+  def __init__(self, T, B, dim_x, dim_err, device):
+    assert T >= 1
+    kw = dict(dtype=torch.float64, device=device)
+    self.T, self.B = int(T), int(B)
+    self.x_pred = torch.empty(T, B, dim_x, **kw)
+    self.x_filt = torch.empty(T, B, dim_x, **kw)
+    self.P_pred = torch.empty(T, B, dim_err, dim_err, **kw)
+    self.P_filt = torch.empty(T, B, dim_err, dim_err, **kw)
+    self.t = torch.zeros(T, B, **kw)
+    self.n = torch.zeros(B, dtype=torch.int32, device=device)
+    self.overflow = torch.zeros((), dtype=torch.int64, device=device)
+
+  def reserve(self, ids, t):
+    """Hand each filter in `ids` (distinct, [m]) its next row, store its time t (scalar or [m]) there and count the row.
+    Returns the rows ([m] int32, on the history's device), -1 for filters that had no row left (counted in overflow)."""
+    dev = self.n.device
+    ids = torch.as_tensor(ids, device=dev).to(torch.int64)
+    t = torch.as_tensor(t, dtype=torch.float64, device=dev).expand(ids.shape[0])
+    k = self.n[ids]
+    full = k >= self.T
+    kc = k.clamp(max=self.T - 1).to(torch.int64)
+    self.t[kc, ids] = torch.where(full, self.t[kc, ids], t)
+    self.n[ids] = k + (~full).to(torch.int32)
+    self.overflow += full.sum()
+    return torch.where(full, -1, k).to(torch.int32)
+
+  def overflowed(self):
+    """Steps not recorded because their filter's rows were used up (synchronises with the device)."""
+    return int(self.overflow)
+
+  def bytes(self):
+    return sum(t.numel() * t.element_size() for t in (self.x_pred, self.x_filt, self.P_pred, self.P_filt, self.t, self.n))

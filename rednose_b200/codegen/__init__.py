@@ -337,6 +337,12 @@ def gen_code(folder, name, f_sym, dt_sym, x_sym, obs_eqs, dim_x, dim_err, eskf_p
     bi = bs.replace(", void *stream", ", const int *idx, void *stream")
     hdr.append(f"void {name}_batch_step_{k}_idx({bi});")
     c.append(f'extern "C" void {name}_batch_step_{k}_idx({bi}) {{ rnb::batch_step<{model}, {ks}, true>(ctx_(), x, P, Q, dt_arr, dt, z, R, ea, n_obs, B, quat_idxs, n_quat, flags, hx_pred, hP_pred, hx_filt, hP_filt, stream, idx); }}\n')
+    # ragged history: entry e records at row hist_row[e] of [T, hist_B, ...] slabs.  Returns the call's cudaError_t (an
+    # int, so the reference-compatible set of `void ` prototypes is unchanged), and its name ends in _idx like its
+    # sibling, so readers that list the kinds from the <name>_batch_step_<kind> symbols skip both.
+    bh = bi.replace(", void *stream", ", const int *hist_row, long long hist_B, void *stream")
+    hdr.append(f"int {name}_batch_step_{k}_hist_idx({bh});")
+    c.append(f'extern "C" int {name}_batch_step_{k}_hist_idx({bh}) {{ return rnb::call_status([&] {{ rnb::batch_step_hist<{model}, {ks}>(ctx_(), x, P, Q, dt_arr, dt, z, R, ea, n_obs, B, quat_idxs, n_quat, flags, hx_pred, hP_pred, hx_filt, hP_filt, idx, hist_row, hist_B, stream); }}); }}\n')
     bm = "const double *x, const double *P, const double *z, const double *R, const double *ea, long long B, int flags, double *out, void *stream"
     hdr.append(f"void {name}_batch_maha_{k}({bm});")
     c.append(f'extern "C" void {name}_batch_maha_{k}({bm}) {{ rnb::batch_maha<{model}, {ks}>(ctx_(), x, P, z, R, ea, B, flags, out, stream); }}\n')
@@ -358,6 +364,10 @@ def gen_code(folder, name, f_sym, dt_sym, x_sym, obs_eqs, dim_x, dim_err, eskf_p
   brs = br.replace(", void *stream", ", const double *x_term, const double *P_term, long long k0, void *stream")
   hdr.append(f"void {name}_batch_rts_segment({brs});")
   c.append(f'extern "C" void {name}_batch_rts_segment({brs}) {{ rnb::batch_rts<{model}>(ctx_(), hx_pred, hP_pred, hx_filt, hP_filt, t, t_per_filter, xs, Ps, T, B, quat_idxs, n_quat, norm_quats, stream, x_term, P_term, k0); }}\n')
+  # ragged history: filter b smooths its first len[b] rows, times t [T, B]; returns the call's cudaError_t (see _hist_idx)
+  brr = "const double *hx_pred, const double *hP_pred, const double *hx_filt, const double *hP_filt, const double *t, const int *len, double *xs, double *Ps, int T, long long B, const int *quat_idxs, int n_quat, int norm_quats, void *stream"
+  hdr.append(f"int {name}_batch_rts_ragged({brr});")
+  c.append(f'extern "C" int {name}_batch_rts_ragged({brr}) {{ return rnb::call_status([&] {{ rnb::batch_rts_ragged<{model}>(ctx_(), hx_pred, hP_pred, hx_filt, hP_filt, t, len, xs, Ps, T, B, quat_idxs, n_quat, norm_quats, stream); }}); }}\n')
 
   if msckf:
     ba = "double *x, double *P, long long B, void *stream"

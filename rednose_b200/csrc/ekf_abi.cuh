@@ -117,9 +117,17 @@ inline void launch_step(const StepArgs<M::NG>& a, cudaStream_t st) {
   }
   // feature-track kinds (left-null-space projection with He, ekf_c.c:66-76) exist only in the CTA kernel: they go there
   // whatever the state size
+  // per-entry history rows come only with the fused gather step (batch_step_hist): the thread and CTA kernels take them
+  // through their own instantiation, the warp kernels on their gather path
+  constexpr bool FUSED = PRED && UPD;
   if constexpr (M::EDIM <= THREAD_MAX_EDIM && !K::HAS_HE) {
     const unsigned grid = (unsigned)((a.B + 127) / 128);
-    ekf_step_thread<M, K, PRED, UPD><<<grid, 128, 0, st>>>(a);
+    if constexpr (FUSED) {
+      if (a.hist_row) ekf_step_thread<M, K, PRED, UPD, true><<<grid, 128, 0, st>>>(a);
+      else ekf_step_thread<M, K, PRED, UPD><<<grid, 128, 0, st>>>(a);
+    } else {
+      ekf_step_thread<M, K, PRED, UPD><<<grid, 128, 0, st>>>(a);
+    }
   } else if constexpr (M::EDIM <= 32 && !K::HAS_HE) {
     if (use_tma<M>() && (reinterpret_cast<uintptr_t>(a.P) & 15u)) {
       fprintf(stderr, "[rednose_b200] P must be 16-byte aligned (bulk-copy staging of covariance tiles)\n");
@@ -184,7 +192,12 @@ inline void launch_step(const StepArgs<M::NG>& a, cudaStream_t st) {
       }
     }
   } else {
-    launch_step_cta<M, K, PRED, UPD>(a, st);
+    if constexpr (FUSED) {
+      if (a.hist_row) launch_step_cta<M, K, PRED, UPD, true>(a, st);
+      else launch_step_cta<M, K, PRED, UPD>(a, st);
+    } else {
+      launch_step_cta<M, K, PRED, UPD>(a, st);
+    }
   }
   check(cudaGetLastError(), "ekf_step launch");
 }
@@ -220,14 +233,31 @@ inline void batch_step(HostCtx<M>& ctx, double* x, double* P, const double* Q, c
                        double* z, const double* R, const double* ea, int n_obs, long long B,
                        const int* quat_idxs, int n_quat, int flags,
                        double* hx_pred, double* hP_pred, double* hx_filt, double* hP_filt, void* stream,
-                       const int* idx = nullptr) {
+                       const int* idx = nullptr, const int* hist_row = nullptr, long long hist_B = 0) {
   StepArgs<M::NG> a;
   if (!fill_common<M>(a, ctx, B, quat_idxs, n_quat, flags)) return;
   a.idx = idx;
+  a.hist_row = hist_row; a.hist_B = hist_B;
   a.x = x; a.P = P; a.Q = Q; a.dt_arr = dt_arr; a.dt = dt;
   a.z = z; a.R = R; a.ea = (K::EADIM > 0) ? ea : nullptr; a.ea_dim = K::EADIM; a.n_obs = n_obs;
   a.hx_pred = hx_pred; a.hP_pred = hP_pred; a.hx_filt = hx_filt; a.hP_filt = hP_filt;
   launch_step<M, K, PRED, true>(a, (cudaStream_t)stream);
+}
+
+// fused gather step that records entry e at row hist_row[e] of [T, hist_B, ...] history slabs (ragged histories)
+template <class M, class K>
+inline void batch_step_hist(HostCtx<M>& ctx, double* x, double* P, const double* Q, const double* dt_arr, double dt,
+                            double* z, const double* R, const double* ea, int n_obs, long long B,
+                            const int* quat_idxs, int n_quat, int flags,
+                            double* hx_pred, double* hP_pred, double* hx_filt, double* hP_filt,
+                            const int* idx, const int* hist_row, long long hist_B, void* stream) {
+  if (!idx || !hist_row || hist_B <= 0) {
+    fprintf(stderr, "[rednose_b200] batch_step_hist: a gather list, its history rows and a positive slab stride are required\n");
+    last_status() = (int)cudaErrorInvalidValue;
+    return;
+  }
+  batch_step<M, K, true>(ctx, x, P, Q, dt_arr, dt, z, R, ea, n_obs, B, quat_idxs, n_quat, flags,
+                         hx_pred, hP_pred, hx_filt, hP_filt, stream, idx, hist_row, hist_B);
 }
 
 }  // namespace rnb
@@ -259,6 +289,32 @@ inline void batch_rts(HostCtx<M>& ctx, const double* hx_pred, const double* hP_p
   a.x_term = (x_term && P_term) ? x_term : nullptr; a.P_term = (x_term && P_term) ? P_term : nullptr; a.k0 = k0;
   a.hx_pred = hx_pred; a.hP_pred = hP_pred; a.hx_filt = hx_filt; a.hP_filt = hP_filt;
   a.t = t; a.t_per_filter = t_per_filter; a.xs = xs; a.Ps = Ps; a.T = T; a.B = B; a.norm_quats = norm_quats;
+  a.n_quat = n_quat;
+  for (int i = 0; i < n_quat; ++i) a.quat_idx[i] = quat_idxs[i];
+  for (int i = 0; i < (M::NG > 0 ? M::NG : 1); ++i) a.gv[i] = ctx.gv.v[i];
+  launch_rts_auto<M>(a, (cudaStream_t)stream);
+}
+
+// RTS over a ragged history: filter b smooths rows 0 .. len[b] - 1 of [T, B, ...] slabs with its own times t [T, B]
+template <class M>
+inline void batch_rts_ragged(HostCtx<M>& ctx, const double* hx_pred, const double* hP_pred, const double* hx_filt, const double* hP_filt,
+                             const double* t, const int* len, double* xs, double* Ps, int T, long long B,
+                             const int* quat_idxs, int n_quat, int norm_quats, void* stream) {
+  if (M::EDIM > 32) {
+    fprintf(stderr, "[rednose_b200] batched RTS for EDIM=%d > 32 is not built into this library\n", M::EDIM);
+    last_status() = (int)cudaErrorNotSupported;
+    return;
+  }
+  if (!t || !len || T <= 0) {
+    fprintf(stderr, "[rednose_b200] batch_rts_ragged: per-filter times, per-filter lengths and T >= 1 are required\n");
+    last_status() = (int)cudaErrorInvalidValue;
+    return;
+  }
+  if (!check_quat_idxs(quat_idxs, n_quat, M::DIM)) return;
+  RtsArgs<M::NG> a;
+  memset(&a, 0, sizeof(a));
+  a.hx_pred = hx_pred; a.hP_pred = hP_pred; a.hx_filt = hx_filt; a.hP_filt = hP_filt;
+  a.t = t; a.t_per_filter = 1; a.len = len; a.xs = xs; a.Ps = Ps; a.T = T; a.B = B; a.norm_quats = norm_quats;
   a.n_quat = n_quat;
   for (int i = 0; i < n_quat; ++i) a.quat_idx[i] = quat_idxs[i];
   for (int i = 0; i < (M::NG > 0 ? M::NG : 1); ++i) a.gv[i] = ctx.gv.v[i];

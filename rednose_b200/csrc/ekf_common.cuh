@@ -53,7 +53,20 @@ struct StepArgs {
   double* hx_filt;       // [B, DIM]        x_{k|k}
   double* hP_filt;       // [B, EDIM, EDIM] P_{k|k}
   double gv[NG > 0 ? NG : 1];
+  // ragged histories (gather list only): entry e records at slab element hist_row[e] * hist_B + idx[e] instead of
+  // idx[e]; a negative row steps without recording.  nullptr = the slabs are indexed by filter.  Kept behind the
+  // existing fields so that the launches without a gather list see the argument block they always had.
+  const int* hist_row;
+  long long hist_B;      // filter stride of the history slabs
 };
+
+// slab element entry e of a gather list records at (-1: nothing recorded)
+template <int NG>
+__device__ __forceinline__ long long hist_slot(const StepArgs<NG>& a, long long e, long long fid) {
+  if (!a.hist_row) return fid;
+  const int r = a.hist_row[e];
+  return r < 0 ? -1 : (long long)r * a.hist_B + fid;
+}
 
 // ---------------------------------------------------------------------------
 // Small symmetric solve used for S = H P H^T + R (ZDIM <= ~8 here).
@@ -173,6 +186,18 @@ inline bool check(cudaError_t e, const char* what) {
   fprintf(stderr, "[rednose_b200] CUDA failure in %s: %s\n", what, cudaGetErrorString(e));
   if (getenv("REDNOSE_B200_ABORT_ON_ERROR")) abort();
   return false;
+}
+
+// Runs an entry point and returns the cudaError_t it latched (0 = ok).  A status latched before the call is kept when the
+// call succeeds, so <name>_cuda_status() still reports it.
+template <class F>
+inline int call_status(F&& f) {
+  const int before = last_status();
+  last_status() = 0;
+  f();
+  const int st = last_status();
+  if (st == 0) last_status() = before;
+  return st;
 }
 
 // The quaternion index list is copied into every launch's argument block and dereferenced in shared memory by the

@@ -37,7 +37,8 @@ struct CtaWs {  // per-filter workspace record (doubles)
 };
 
 // ------------------------------------------------------------------ leaf kernel ---
-template <class M, class K, bool PRED, bool UPD>
+// HIST (both kernels): gather list with per-entry history rows (StepArgs::hist_row)
+template <class M, class K, bool PRED, bool UPD, bool HIST = false>
 __global__ void __launch_bounds__(64) ekf_leaf_thread(const StepArgs<M::NG> a, int o, double* __restrict__ ws_all) {
   constexpr int D = M::DIM, Z = K::ZDIM;
   using W = CtaWs<M, K>;
@@ -45,6 +46,8 @@ __global__ void __launch_bounds__(64) ekf_leaf_thread(const StepArgs<M::NG> a, i
   if (b >= a.B) return;
   double* ws = ws_all + b * W::SIZE;
   const long long fb = a.idx ? (long long)a.idx[b] : b;   // filter this entry works on
+  long long hb = fb;                                       // history slab element of this entry (-1: not recorded)
+  if constexpr (HIST) hb = hist_slot(a, b, fb);
   double x[D];
   if (PRED || o == 0) {
 #pragma unroll
@@ -68,9 +71,9 @@ __global__ void __launch_bounds__(64) ekf_leaf_thread(const StepArgs<M::NG> a, i
     }
 #pragma unroll
     for (int i = 0; i < D; ++i) x[i] = ws[W::OFF_X + i];
-    if (a.hx_pred) {
+    if (a.hx_pred && (!HIST || hb >= 0)) {
 #pragma unroll
-      for (int i = 0; i < D; ++i) a.hx_pred[fb * D + i] = x[i];
+      for (int i = 0; i < D; ++i) a.hx_pred[hb * D + i] = x[i];
     }
     if (!UPD) {
 #pragma unroll
@@ -206,7 +209,7 @@ constexpr int cta_threads() { return ((M::EDIM + 31) / 32) * 32; }   // one thre
 #define RNB_CTA_MIN_BLOCKS 4
 #endif
 
-template <class M, class K, bool PRED, bool UPD>
+template <class M, class K, bool PRED, bool UPD, bool HIST = false>
 __global__ void __launch_bounds__(cta_threads<M>(), RNB_CTA_MIN_BLOCKS) ekf_step_cta(const StepArgs<M::NG> a, int o, const double* __restrict__ ws_all) {
   constexpr int D = M::DIM, E = M::EDIM, ME = M::MEDIM, Z = K::ZDIM, Y = K::YDIM, NR = Z - Y;
   using SM = CtaSmem<M, K>;
@@ -221,6 +224,9 @@ __global__ void __launch_bounds__(cta_threads<M>(), RNB_CTA_MIN_BLOCKS) ekf_step
   const long long b = blockIdx.x;
   const double* ws = ws_all + b * W::SIZE;
   const long long fb = a.idx ? (long long)a.idx[b] : b;   // filter this entry works on
+  long long hb = fb;                                       // history slab element of this entry (-1: not recorded)
+  if constexpr (HIST) hb = hist_slot(a, b, fb);
+  const bool rec = !HIST || hb >= 0;
   double* Pg = a.P + fb * (long long)(E * E);
   const bool own = col < E;            // this thread is attached to column `col`
   const PackedCol pc{s.Ppk, own ? col : 0, own ? col * (col + 1) / 2 : 0};
@@ -325,7 +331,7 @@ __global__ void __launch_bounds__(cta_threads<M>(), RNB_CTA_MIN_BLOCKS) ekf_step
       }
     }
     __syncthreads();
-    if (a.hP_pred) store_full(a.hP_pred + fb * (long long)(E * E));
+    if (a.hP_pred && rec) store_full(a.hP_pred + hb * (long long)(E * E));
   }
 
   if constexpr (UPD) {
@@ -508,12 +514,12 @@ __global__ void __launch_bounds__(cta_threads<M>(), RNB_CTA_MIN_BLOCKS) ekf_step
           a.x[fb * D + i] = s.xo[si];
         }
         const_cast<double*>(ws_all)[b * W::SIZE + W::OFF_X + i] = v;  // next observation of this batch starts here
-        if (last && a.hx_filt) a.hx_filt[fb * D + i] = v;              // the history keeps the estimate BEFORE the window shifts (ekf_sym.py:523-528)
+        if (last && a.hx_filt && rec) a.hx_filt[hb * D + i] = v;       // the history keeps the estimate BEFORE the window shifts (ekf_sym.py:523-528)
       }
       // innovation overwrites z (ekf_c.c:120): the first YDIM entries
       for (int i = tid; i < Y; i += 32) a.z[(b * a.n_obs + o) * Z + i] = s.y[NR + i];
     }
-    if (last && a.hP_filt) store_full(a.hP_filt + fb * (long long)(E * E));
+    if (last && a.hP_filt && rec) store_full(a.hP_filt + hb * (long long)(E * E));
   }
 
   if (!aug) {
@@ -533,7 +539,7 @@ __global__ void __launch_bounds__(cta_threads<M>(), RNB_CTA_MIN_BLOCKS) ekf_step
   }
 }
 
-template <class M, class K, bool PRED, bool UPD>
+template <class M, class K, bool PRED, bool UPD, bool HIST = false>
 inline void launch_step_cta(const StepArgs<M::NG>& a, cudaStream_t st) {
   using W = CtaWs<M, K>;
   // leaf-value workspace of THIS call, allocated and released in stream order (calls on different streams / devices
@@ -541,20 +547,20 @@ inline void launch_step_cta(const StepArgs<M::NG>& a, cudaStream_t st) {
   double* ws = (double*)stream_alloc(sizeof(double) * (size_t)a.B * W::SIZE, st, "cudaMallocAsync(cta workspace)");
   if (!ws) return;
   constexpr size_t smem = sizeof(CtaSmem<M, K>);
-  if (first_launch_of((const void*)ekf_step_cta<M, K, PRED, UPD>))
-    check(cudaFuncSetAttribute(ekf_step_cta<M, K, PRED, UPD>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem), "smem attribute");
-  if (first_launch_of((const void*)ekf_step_cta<M, K, false, UPD>))
-    check(cudaFuncSetAttribute(ekf_step_cta<M, K, false, UPD>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem), "smem attribute");
+  if (first_launch_of((const void*)ekf_step_cta<M, K, PRED, UPD, HIST>))
+    check(cudaFuncSetAttribute(ekf_step_cta<M, K, PRED, UPD, HIST>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem), "smem attribute");
+  if (first_launch_of((const void*)ekf_step_cta<M, K, false, UPD, HIST>))
+    check(cudaFuncSetAttribute(ekf_step_cta<M, K, false, UPD, HIST>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem), "smem attribute");
   constexpr int threads = cta_threads<M>();
   const int n_obs = UPD ? a.n_obs : 1;
   for (int o = 0; o < n_obs; ++o) {
     const unsigned lgrid = (unsigned)((a.B + 63) / 64);
     if (o == 0) {
-      ekf_leaf_thread<M, K, PRED, UPD><<<lgrid, 64, 0, st>>>(a, o, ws);
-      ekf_step_cta<M, K, PRED, UPD><<<(unsigned)a.B, threads, smem, st>>>(a, o, ws);
+      ekf_leaf_thread<M, K, PRED, UPD, HIST><<<lgrid, 64, 0, st>>>(a, o, ws);
+      ekf_step_cta<M, K, PRED, UPD, HIST><<<(unsigned)a.B, threads, smem, st>>>(a, o, ws);
     } else {
-      ekf_leaf_thread<M, K, false, UPD><<<lgrid, 64, 0, st>>>(a, o, ws);
-      ekf_step_cta<M, K, false, UPD><<<(unsigned)a.B, threads, smem, st>>>(a, o, ws);
+      ekf_leaf_thread<M, K, false, UPD, HIST><<<lgrid, 64, 0, st>>>(a, o, ws);
+      ekf_step_cta<M, K, false, UPD, HIST><<<(unsigned)a.B, threads, smem, st>>>(a, o, ws);
     }
   }
   check(cudaFreeAsync(ws, st), "cudaFreeAsync(cta workspace)");

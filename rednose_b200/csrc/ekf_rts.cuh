@@ -54,7 +54,18 @@ struct RtsArgs {
   const double* P_term;
   long long k0;
   double gv[NG > 0 ? NG : 1];
+  // ragged histories: filter b smooths rows 0 .. len[b] - 1 only (with t [T, B]) and leaves its rows >= len[b] of xs / Ps
+  // untouched; nullptr = every filter has T rows.  Not combined with segment continuation.
+  const int* len;
 };
+
+// rows filter b smooths: T, or len[b] clamped to [0, T] for a ragged history
+template <bool RAGGED, int NG>
+__device__ __forceinline__ long long rts_rows(const RtsArgs<NG>& a, long long b) {
+  if constexpr (!RAGGED) return a.T;
+  const long long n = a.len[b];
+  return n < 0 ? 0 : (n > a.T ? a.T : n);
+}
 
 constexpr int RTS_WARPS = 2;
 #ifndef RNB_RTS_MIN_CTAS
@@ -77,7 +88,7 @@ struct RtsScratch {
   alignas(16) double dinv[(N + 1) & ~1];              // 1 / D[k]
 };
 
-template <class M>
+template <class M, bool RAGGED = false>
 __global__ void __launch_bounds__(RTS_WARPS * 32, RTS_MIN_CTAS) ekf_rts_warp(const RtsArgs<M::NG> a) {
   constexpr int D = M::DIM, E = M::EDIM, N = M::MEDIM, D1 = M::DMAIN;
   using SC = RtsScratch<M>;
@@ -87,6 +98,8 @@ __global__ void __launch_bounds__(RTS_WARPS * 32, RTS_MIN_CTAS) ekf_rts_warp(con
   const int lane = threadIdx.x & 31, wib = threadIdx.x >> 5;
   const long long b = (long long)blockIdx.x * RTS_WARPS + wib;
   if (b >= a.B) return;
+  const long long T = rts_rows<RAGGED>(a, b);   // warp-uniform; the warps of a CTA never synchronise with each other
+  if (RAGGED && T == 0) return;
   SC& s = s_all[wib];
   const bool act = lane < N;        // owns a column of the main block
   const bool actE = lane < E;       // owns a column of the full covariance
@@ -106,7 +119,7 @@ __global__ void __launch_bounds__(RTS_WARPS * 32, RTS_MIN_CTAS) ekf_rts_warp(con
   // ---- start: x_{T-1|N} = x_{T-1|T-2} (predicted), P likewise (ekf_sym.py:658-659) ----
   double pn[N];  // column `lane` of the carried smoothed covariance (main block)
   {
-    const long long k = a.T - 1;
+    const long long k = T - 1;
     const bool seg = a.x_term != nullptr;
     const double* Pg = (seg ? a.P_term + b * (long long)(E * E) : a.hP_pred + k * BP + b * (long long)(E * E)) + col;
     double* Po = a.Ps + k * BP + b * (long long)(E * E) + col;
@@ -119,13 +132,13 @@ __global__ void __launch_bounds__(RTS_WARPS * 32, RTS_MIN_CTAS) ekf_rts_warp(con
     for (int i = lane; i < D; i += 32) s.xn[i] = seg ? a.x_term[b * D + i] : a.hx_pred[k * BX + b * D + i];
     __syncwarp();
     if (!seg) {
-      if (a.norm_quats && a.T >= 2) normalize_xn();
+      if (a.norm_quats && T >= 2) normalize_xn();
       for (int i = lane; i < D; i += 32) a.xs[k * BX + b * D + i] = s.xn[i];
     }
   }
 
 #pragma unroll 1
-  for (long long k = a.T - 2; k >= 0; --k) {
+  for (long long k = T - 2; k >= 0; --k) {
     const double* Pf_g = a.hP_filt + k * BP + b * (long long)(E * E) + col;
     const double* Pp_g = a.hP_pred + (k + 1) * BP + b * (long long)(E * E) + col;
     double g[N];
@@ -265,7 +278,8 @@ inline void launch_rts(const RtsArgs<M::NG>& a, cudaStream_t st) {
   if (a.B <= 0 || a.T <= 0) return;
   if constexpr (M::EDIM <= 32) {
     const unsigned grid = (unsigned)((a.B + RTS_WARPS - 1) / RTS_WARPS);
-    ekf_rts_warp<M><<<grid, RTS_WARPS * 32, 0, st>>>(a);
+    if (a.len) ekf_rts_warp<M, true><<<grid, RTS_WARPS * 32, 0, st>>>(a);
+    else ekf_rts_warp<M><<<grid, RTS_WARPS * 32, 0, st>>>(a);
     check(cudaGetLastError(), "ekf_rts launch");
   } else {
     fprintf(stderr, "[rednose_b200] batched RTS for EDIM=%d > 32 is not built into this library\n", M::EDIM);

@@ -47,7 +47,7 @@ struct RtsMmaScratch {
   alignas(16) double dinv[(N + 1) & ~1];
 };
 
-template <class M>
+template <class M, bool RAGGED = false>
 __global__ void __launch_bounds__(RTS_WARPS * 32, RTS_MIN_CTAS) ekf_rts_warp_mma(const RtsArgs<M::NG> a) {
   constexpr int D = M::DIM, E = M::EDIM, N = M::MEDIM, D1 = M::DMAIN;
   using SC = RtsMmaScratch<M>;
@@ -59,6 +59,8 @@ __global__ void __launch_bounds__(RTS_WARPS * 32, RTS_MIN_CTAS) ekf_rts_warp_mma
   const int lane = threadIdx.x & 31, wib = threadIdx.x >> 5;
   const long long b = (long long)blockIdx.x * RTS_WARPS + wib;
   if (b >= a.B) return;
+  const long long T = rts_rows<RAGGED>(a, b);   // warp-uniform; the warps of a CTA never synchronise with each other
+  if (RAGGED && T == 0) return;
   SC& s = s_all[wib];
   const bool act = lane < N, actE = lane < E;
   const int col = actE ? lane : 0;
@@ -80,7 +82,7 @@ __global__ void __launch_bounds__(RTS_WARPS * 32, RTS_MIN_CTAS) ekf_rts_warp_mma
   // ---- start: smoothed = predicted at T-1 (ekf_sym.py:658-659); carried in fragment layout ----
   double pn[NT * NT * 2];
   {
-    const long long k = a.T - 1;
+    const long long k = T - 1;
     const bool seg = a.x_term != nullptr;   // segment continuation: start from the smoothed estimate handed in
     const double* Pg = seg ? a.P_term + b * (long long)(E * E) : a.hP_pred + k * BP + b * (long long)(E * E);
     double* Po = a.Ps + k * BP + b * (long long)(E * E);
@@ -97,13 +99,13 @@ __global__ void __launch_bounds__(RTS_WARPS * 32, RTS_MIN_CTAS) ekf_rts_warp_mma
     for (int i = lane; i < D; i += 32) s.xn[i] = seg ? a.x_term[b * D + i] : a.hx_pred[k * BX + b * D + i];
     __syncwarp();
     if (!seg) {
-      if (a.norm_quats && a.T >= 2) normalize_xn();
+      if (a.norm_quats && T >= 2) normalize_xn();
       for (int i = lane; i < D; i += 32) a.xs[k * BX + b * D + i] = s.xn[i];
     }
   }
 
 #pragma unroll 1
-  for (long long k = a.T - 2; k >= 0; --k) {
+  for (long long k = T - 2; k >= 0; --k) {
     const double* Pf_b = a.hP_filt + k * BP + b * (long long)(E * E);
     const double* Pp_b = a.hP_pred + (k + 1) * BP + b * (long long)(E * E);
     const double* Pf_g = Pf_b + col;
@@ -301,13 +303,20 @@ __global__ void __launch_bounds__(RTS_WARPS * 32, RTS_MIN_CTAS) ekf_rts_warp_mma
 
 template <class M>
 inline void launch_rts_auto(const RtsArgs<M::NG>& a, cudaStream_t st) {
+  if (a.len && a.x_term) {
+    fprintf(stderr, "[rednose_b200] RTS: per-filter lengths and segment continuation cannot be combined\n");
+    last_status() = (int)cudaErrorNotSupported;
+    return;
+  }
   if (a.B <= 0 || a.T <= 0) return;
   if constexpr (RNB_RTS_MMA && M::EDIM <= 32 && M::EDIM % 2 == 0 && M::MEDIM >= 8) {
     const unsigned grid = (unsigned)((a.B + RTS_WARPS - 1) / RTS_WARPS);
     constexpr size_t smem = sizeof(RtsMmaScratch<M>) * RTS_WARPS;   // 55 296 B at EDIM 32, 32 192 B for live_kf
-    if (first_launch_of((const void*)ekf_rts_warp_mma<M>))
-      cudaFuncSetAttribute(ekf_rts_warp_mma<M>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    ekf_rts_warp_mma<M><<<grid, RTS_WARPS * 32, smem, st>>>(a);
+    auto run = [&](void (*kern)(const RtsArgs<M::NG>)) {
+      if (first_launch_of((const void*)kern)) cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+      kern<<<grid, RTS_WARPS * 32, smem, st>>>(a);
+    };
+    run(a.len ? ekf_rts_warp_mma<M, true> : ekf_rts_warp_mma<M, false>);
     check(cudaGetLastError(), "ekf_rts_mma launch");
   } else {
     launch_rts<M>(a, st);

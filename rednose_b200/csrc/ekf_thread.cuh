@@ -39,13 +39,17 @@ __device__ __forceinline__ void store_rec(double* __restrict__ g, const double (
   }
 }
 
-template <class M, class K, bool PRED, bool UPD>
+// HIST: gather list with per-entry history rows (StepArgs::hist_row); the other instantiations are the kernel as it was
+template <class M, class K, bool PRED, bool UPD, bool HIST = false>
 __global__ void __launch_bounds__(128) ekf_step_thread(const StepArgs<M::NG> a) {
   constexpr int D = M::DIM, E = M::EDIM, Z = K::ZDIM;
   const long long b = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (b >= a.B) return;
 
   const long long fb = a.idx ? (long long)a.idx[b] : b;   // filter this entry works on
+  long long hb = fb;                                       // history slab element of this entry (-1: not recorded)
+  if constexpr (HIST) hb = hist_slot(a, b, fb);
+  const bool rec = !HIST || hb >= 0;
   double x[D];
   double P[E * E];
   load_rec<D>(a.x + fb * D, x);
@@ -96,8 +100,8 @@ __global__ void __launch_bounds__(128) ekf_step_thread(const StepArgs<M::NG> a) 
 #pragma unroll
           for (int i = 0; i < D; ++i) if (i == a.quat_idx[q] + c) x[i] = qv[c];
       }
-    if (a.hx_pred) store_rec<D>(a.hx_pred + fb * D, x);
-    if (a.hP_pred) store_rec<E * E>(a.hP_pred + fb * E * E, P);
+    if (a.hx_pred && rec) store_rec<D>(a.hx_pred + hb * D, x);
+    if (a.hP_pred && rec) store_rec<E * E>(a.hP_pred + hb * E * E, P);
   }
 
   if constexpr (UPD) {
@@ -209,8 +213,8 @@ __global__ void __launch_bounds__(128) ekf_step_thread(const StepArgs<M::NG> a) 
 #pragma unroll
       for (int i = 0; i < Z; ++i) a.z[bo * Z + i] = y[i];
     }
-    if (a.hx_filt) store_rec<D>(a.hx_filt + fb * D, x);
-    if (a.hP_filt) store_rec<E * E>(a.hP_filt + fb * E * E, P);
+    if (a.hx_filt && rec) store_rec<D>(a.hx_filt + hb * D, x);
+    if (a.hP_filt && rec) store_rec<E * E>(a.hP_filt + hb * E * E, P);
   }
 
   store_rec<D>(a.x + fb * D, x);

@@ -106,6 +106,7 @@ struct RowLayout {
   static constexpr int OFF_R = OFF_Y + Zp;          // measurement noise
   static constexpr int OFF_X = OFF_R + ZZp;         // predicted state
   static constexpr int OFF_DT = OFF_X + Dp;         // dt of this filter (+1 pad)
+  static constexpr int OFF_HID = OFF_DT + 1;        // the pad: history slab element of a gather entry (ekf_step_pair)
   static constexpr int RAW = OFF_DT + 2;
   static constexpr int STRIDE = RAW + ((2 - RAW % 4) + 4) % 4;  // = 2 (mod 4)
 };
@@ -192,15 +193,15 @@ __device__ __forceinline__ void stage_out(double* __restrict__ g, const double* 
   }
 }
 
-// scattered counterpart of stage_out
-template <int WD, int STRIDE>
+// scattered counterpart of stage_out; with SKIP_NEG a record whose destination index is negative is not written
+template <int WD, int STRIDE, bool SKIP_NEG = false>
 __device__ __forceinline__ void scatter_out(double* __restrict__ g, const double* rows, int off, int ng, int lane, long long myfid) {
   for (int base = 0; base < ng * WD; base += 32) {
     const int idx = base + lane;
     const bool ok = idx < ng * WD;
     const int f = ok ? idx / WD : 0, i = idx - f * WD;
     const long long fid = __shfl_sync(0xffffffffu, myfid, f);
-    if (ok) g[fid * WD + i] = rows[f * STRIDE + off + i];
+    if (ok && (!SKIP_NEG || fid >= 0)) g[fid * WD + i] = rows[f * STRIDE + off + i];
   }
 }
 
@@ -230,12 +231,20 @@ __global__ void __launch_bounds__(W * 32, RNB_MIN_WARPS / W) ekf_step_warp(const
   // filter this lane's entry works on (gather list, ragged scheduler) -- entry index when there is no list
   constexpr bool gathered = GATHER;
   long long myfid = b0 + (mine ? lane : 0);
-  if constexpr (GATHER) { if (mine) myfid = (long long)a.idx[b0 + lane]; }
+  long long myhid = 0;       // gather lists: history slab element of this lane's entry (-1: not recorded)
+  if constexpr (GATHER) {
+    myhid = myfid;
+    if (mine) {
+      myfid = (long long)a.idx[b0 + lane];
+      myhid = hist_slot(a, b0 + lane, myfid);
+    }
+  }
   // filter id of entry f of the group: a shuffle only when a gather list is in use
   auto fid_of = [&](int f) -> long long {
     if constexpr (GATHER) return __shfl_sync(0xffffffffu, myfid, f);
     else return b0 + f;
   };
+  auto hid_of = [&](int f) -> long long { return __shfl_sync(0xffffffffu, myhid, f); };   // gather lists only
 
   constexpr bool TMA = use_tma<M>();
   constexpr int NST = TMA ? RNB_STAGES : 1;
@@ -354,7 +363,7 @@ __global__ void __launch_bounds__(W * 32, RNB_MIN_WARPS / W) ekf_step_warp(const
     }
     __syncwarp();
     if (do_pred && a.hx_pred) {
-      if (gathered) scatter_out<D, RS>(a.hx_pred, s.rows, L::OFF_X, ng, lane, myfid);
+      if (gathered) scatter_out<D, RS, true>(a.hx_pred, s.rows, L::OFF_X, ng, lane, myhid);
       else stage_out<D, RS>(a.hx_pred + b0 * D, s.rows, L::OFF_X, ng, lane);
     }
     if constexpr (UPD) {
@@ -372,6 +381,9 @@ __global__ void __launch_bounds__(W * 32, RNB_MIN_WARPS / W) ekf_step_warp(const
 #pragma unroll 1
     for (int f = 0; f < ng; ++f) {
       const long long b = fid_of(f);   // filter id of this iteration
+      long long hb = b;                // its history slab element
+      bool rec = true;
+      if constexpr (GATHER) { hb = hid_of(f); rec = hb >= 0; }
       double* row = s.rows + f * RS;
       double p[E];
       const uint32_t slot = it % NST;
@@ -462,8 +474,8 @@ __global__ void __launch_bounds__(W * 32, RNB_MIN_WARPS / W) ekf_step_warp(const
 #pragma unroll
           for (int i = 0; i < E; ++i) p[i] = fma(dt, __ldg(Qg + i * E), p[i]);
         }
-        if (a.hP_pred && act) {
-          double* Hg = a.hP_pred + b * (long long)(E * E) + col;
+        if (a.hP_pred && act && rec) {
+          double* Hg = a.hP_pred + hb * (long long)(E * E) + col;
 #pragma unroll
           for (int i = 0; i < E; ++i) Hg[i * E] = p[i];
         }
@@ -537,8 +549,8 @@ __global__ void __launch_bounds__(W * 32, RNB_MIN_WARPS / W) ekf_step_warp(const
           if (i + 1 < E) p[i + 1] = a1;
         }
         __syncwarp();
-        if (a.hP_filt && act && o == n_obs - 1) {
-          double* Hg = a.hP_filt + b * (long long)(E * E) + col;
+        if (a.hP_filt && act && rec && o == n_obs - 1) {
+          double* Hg = a.hP_filt + hb * (long long)(E * E) + col;
 #pragma unroll
           for (int i = 0; i < E; ++i) Hg[i * E] = p[i];
         }
@@ -577,7 +589,7 @@ __global__ void __launch_bounds__(W * 32, RNB_MIN_WARPS / W) ekf_step_warp(const
       if (gathered) scatter_out<D, RS>(a.x, s.rows, L::OFF_X, ng, lane, myfid);
       else stage_out<D, RS>(a.x + b0 * D, s.rows, L::OFF_X, ng, lane);
       if (UPD && a.hx_filt) {
-        if (gathered) scatter_out<D, RS>(a.hx_filt, s.rows, L::OFF_X, ng, lane, myfid);
+        if (gathered) scatter_out<D, RS, true>(a.hx_filt, s.rows, L::OFF_X, ng, lane, myhid);
         else stage_out<D, RS>(a.hx_filt + b0 * D, s.rows, L::OFF_X, ng, lane);
       }
     }

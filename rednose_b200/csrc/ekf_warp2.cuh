@@ -103,11 +103,20 @@ __global__ void __launch_bounds__(32, RNB_PAIR_MIN_WARPS) ekf_step_pair(const St
   double* myrow = s.rows + (lane < G ? lane : 0) * RS;
   const bool mine = lane < ng;
   long long myfid = b0 + (mine ? lane : 0);
-  if constexpr (GATHER) { if (mine) myfid = (long long)a.idx[b0 + lane]; }
+  if constexpr (GATHER) {
+    if (mine) {
+      myfid = (long long)a.idx[b0 + lane];
+      // the entry's history slab element waits in its row (no register held through the kernel: the gather
+      // instantiations are at the 8-warps-per-SM register limit)
+      *reinterpret_cast<long long*>(myrow + L::OFF_HID) = hist_slot(a, b0 + lane, myfid);
+    }
+  }
   auto fid_of = [&](int f) -> long long {
     if constexpr (GATHER) return __shfl_sync(0xffffffffu, myfid, f);
     else return b0 + f;
   };
+  // gather lists: history slab element of this lane's entry (-1: not recorded)
+  auto my_hid = [&]() -> long long { return mine ? *reinterpret_cast<const long long*>(myrow + L::OFF_HID) : 0; };
   double* exh = s.exhp + h * XN;            // this half's exchange / (H P) buffer
 
   constexpr int NST = SC::NST;
@@ -284,7 +293,7 @@ __global__ void __launch_bounds__(32, RNB_PAIR_MIN_WARPS) ekf_step_pair(const St
     }
     __syncwarp();
     if (do_pred && a.hx_pred) {
-      if (GATHER) scatter_out<D, RS>(a.hx_pred, s.rows, L::OFF_X, ng, lane, myfid);
+      if (GATHER) scatter_out<D, RS, true>(a.hx_pred, s.rows, L::OFF_X, ng, lane, my_hid());
       else stage_out<D, RS>(a.hx_pred + b0 * D, s.rows, L::OFF_X, ng, lane);
     }
     if constexpr (UPD) {
@@ -304,6 +313,9 @@ __global__ void __launch_bounds__(32, RNB_PAIR_MIN_WARPS) ekf_step_pair(const St
       const int fi = valid ? f + h : f;
       const bool wr = valid && act;
       const long long b = fid_of(fi);
+      // gather lists: history slab element of this half's filter, read from its row where it is stored at each use (a
+      // register held across the iteration spills)
+      auto hist_el = [&]() -> long long { return *reinterpret_cast<const long long*>(s.rows + fi * RS + L::OFF_HID); };
       double* row = s.rows + fi * RS;
       const uint32_t slot = it % NST;
       const double* tile = s.tile + slot * (2 * TS) + (valid ? h : 0) * TS;
@@ -403,7 +415,11 @@ __global__ void __launch_bounds__(32, RNB_PAIR_MIN_WARPS) ekf_step_pair(const St
             p1[i] = fma(dt, __ldg(Qg + i * E + 1), p1[i]);
           }
         }
-        if (a.hP_pred && wr) store_cols(a.hP_pred + b * (long long)(E * E), p0, p1);
+        if constexpr (GATHER) {
+          const long long hb = hist_el();
+          if (a.hP_pred && wr && hb >= 0) store_cols(a.hP_pred + hb * (long long)(E * E), p0, p1);
+        }
+        else { if (a.hP_pred && wr) store_cols(a.hP_pred + b * (long long)(E * E), p0, p1); }
       }
 
       if constexpr (UPD) {
@@ -478,13 +494,18 @@ __global__ void __launch_bounds__(32, RNB_PAIR_MIN_WARPS) ekf_step_pair(const St
           p0[i] = a0; p0[i + 1] = a1; p1[i] = b0v; p1[i + 1] = b1v;
         }
         __syncwarp();
-        if (a.hP_filt && wr && o == n_obs - 1) store_full(a.hP_filt + b * (long long)(E * E), p0, p1);   // = the state, bit for bit
+        if constexpr (!GATHER) { if (a.hP_filt && wr && o == n_obs - 1) store_full(a.hP_filt + b * (long long)(E * E), p0, p1); }   // = the state, bit for bit
+        else {
+          const long long hb = hist_el();
+          if (a.hP_filt && wr && hb >= 0 && o == n_obs - 1) store_full(a.hP_filt + hb * (long long)(E * E), p0, p1);
+        }
       }
 
+      const long long bp = GATHER ? fid_of(fi) : b;   // gather lists: shuffled again here rather than held through the update
       if (wr) {
         if constexpr (PACKED) {
           // the lane's blocks (I, hl), I >= hl: one 32-byte block per iteration, two 128-bit stores
-          double* Pg = a.P + b * (long long)TS;
+          double* Pg = a.P + bp * (long long)TS;
 #pragma unroll
           for (int I = 0; I < E / 2; ++I) {
             if (I >= hl) {
@@ -494,7 +515,7 @@ __global__ void __launch_bounds__(32, RNB_PAIR_MIN_WARPS) ekf_step_pair(const St
             }
           }
         } else {
-          store_full(a.P + b * (long long)(E * E), p0, p1);
+          store_full(a.P + bp * (long long)(E * E), p0, p1);
         }
       }
     }
@@ -517,7 +538,7 @@ __global__ void __launch_bounds__(32, RNB_PAIR_MIN_WARPS) ekf_step_pair(const St
       if (GATHER) scatter_out<D, RS>(a.x, s.rows, L::OFF_X, ng, lane, myfid);
       else stage_out<D, RS>(a.x + b0 * D, s.rows, L::OFF_X, ng, lane);
       if (UPD && a.hx_filt) {
-        if (GATHER) scatter_out<D, RS>(a.hx_filt, s.rows, L::OFF_X, ng, lane, myfid);
+        if (GATHER) scatter_out<D, RS, true>(a.hx_filt, s.rows, L::OFF_X, ng, lane, my_hid());
         else stage_out<D, RS>(a.hx_filt + b0 * D, s.rows, L::OFF_X, ng, lane);
       }
     }
