@@ -99,7 +99,7 @@ __global__ void __launch_bounds__(RTS_WARPS * 32, RTS_MIN_CTAS) ekf_rts_warp_mma
     for (int i = lane; i < D; i += 32) s.xn[i] = seg ? a.x_term[b * D + i] : a.hx_pred[k * BX + b * D + i];
     __syncwarp();
     if (!seg) {
-      if (a.norm_quats && T >= 2) normalize_xn();
+      if (a.norm_quats && a.k0 + T - 1 >= 1) normalize_xn();   // every output but global index 0, as in the loop
       for (int i = lane; i < D; i += 32) a.xs[k * BX + b * D + i] = s.xn[i];
     }
   }

@@ -202,7 +202,13 @@ class HiPrecModel:
     return x, P, (ys if isinstance(z, list) else ys[0])
 
   def rts(self, x_pred, x_filt, P_pred, P_filt, t, norm_quats=False, quat_idxs=(3,)):
-    """oracle/rts_numpy.rts_smooth for one filter (lists of mp matrices); returns (xs, Ps) in time order."""
+    """oracle/rts_numpy.rts_smooth for one filter (lists of mp matrices); returns (xs, Ps) in time order.
+
+    With ``msckf_params`` only the main block is smoothed (ekf_sym.py:651-690 with dim_main / dim_main_err): C is formed
+    from the main blocks of F, P_{k|k} and P_{k+1|k}, only delta[:d2] of the full inv_err delta is replaced by C delta[:d2],
+    x_{k|N} is x_{k|k} with [:d1] taken from err_fun(x_{k|k}, delta), and P_{k|N} is P_{k|k} with the main block
+    replaced.  Every quaternion in `quat_idxs` is normalised, clones included."""
+    d1, d2 = (self.msckf[0], self.msckf[2]) if self.msckf else (self.dim_x, self.dim_err)
     T = len(x_pred)
     xk_n, Pk_n = x_pred[-1].copy(), P_pred[-1].copy()
     xs, Ps = [xk_n], [Pk_n]
@@ -212,10 +218,22 @@ class HiPrecModel:
         xs[-1] = xk1_n
       Pk1_n = Pk_n
       xk1_k, Pk1_k, xk_k, Pk_k = x_pred[k + 1], P_pred[k + 1], x_filt[k], P_filt[k]
-      F = self.F(xk_k, t[k + 1] - t[k])
-      C = _mul(mp.inverse(Pk1_k), _mul(F, Pk_k.T)).T              # solve(Pk1_k, F Pk_k^T)^T
-      xk_n = self.err_fun(xk_k, C * self.inv_err_fun(xk1_k, xk1_n))
-      Pk_n = Pk_k + _mul(_mul(C, Pk1_n - Pk1_k), C.T)
+      F = _block(self.F(xk_k, t[k + 1] - t[k]), d2)
+      Pk1_k_m, Pk_k_m = _block(Pk1_k, d2), _block(Pk_k, d2)
+      C = _mul(mp.inverse(Pk1_k_m), _mul(F, Pk_k_m.T)).T          # solve(Pk1_k, F Pk_k^T)^T on the main block
+      delta = self.inv_err_fun(xk1_k, xk1_n)
+      cd = C * mp.matrix([delta[i] for i in range(d2)])
+      for i in range(d2):
+        delta[i] = cd[i]
+      xe = self.err_fun(xk_k, delta)
+      xk_n = xk_k.copy()
+      for i in range(d1):
+        xk_n[i] = xe[i]
+      Pm = Pk_k_m + _mul(_mul(C, _block(Pk1_n, d2) - Pk1_k_m), C.T)
+      Pk_n = Pk_k.copy()
+      for i in range(d2):
+        for j in range(d2):
+          Pk_n[i, j] = Pm[i, j]
       xs.append(xk_n)
       Ps.append(Pk_n)
     return xs[::-1], Ps[::-1]
@@ -227,13 +245,15 @@ class HiPrecModel:
     conv = [np.asarray(a, dtype=np.float64).reshape(-1, 1) if np.ndim(a) else float(a) for a in args]
     return np.array(self._fn(key, "numpy")(*conv, *self.gv), dtype=np.float64).reshape(-1)
 
-  def step_f64(self, kind, x, P, Q, dt, z, R, quat_idxs=(), flags=3, ea=None):
-    """Fused step in float64 (no gate, Joseph form), x [DIM], P [E, E]; returns (x, P, y)."""
+  def step_f64(self, kind, x, P, Q, dt, z, R, quat_idxs=(), flags=3, ea=None, predict=True):
+    """Fused step in float64 (no gate, Joseph form), x [DIM], P [E, E]; returns (x, P, y).  predict=False: the update
+    alone (Q, dt unused)."""
     E, D = self.dim_err, self.dim_x
-    F = self.np_leaf('F', x, dt).reshape(E, E)
-    x = self.np_leaf('f', x, dt)
-    P = F @ P @ F.T + dt * Q
-    if flags & 1:
+    if predict:
+      F = self.np_leaf('F', x, dt).reshape(E, E)
+      x = self.np_leaf('f', x, dt)
+      P = F @ P @ F.T + dt * Q
+    if predict and flags & 1:
       x = _np_normalize(x, quat_idxs)
     ea_args = [ea] if ea is not None else []
     He = self.np_leaf(('H', kind), x, *ea_args).reshape(self.zdim[kind], D) @ self.np_leaf('H_mod', x).reshape(D, E)
@@ -270,6 +290,17 @@ def _mul(A, B):
       for j in range(B.cols):
         c = cols[j]
         out[i, j] = mp.fdot((a, c[k]) for k, a in nz)
+  return out
+
+
+def _block(A, n):
+  """The leading n x n block of an mp matrix (A itself when it is n x n)."""
+  if A.rows == n and A.cols == n:
+    return A
+  out = mp.matrix(n, n)
+  for i in range(n):
+    for j in range(n):
+      out[i, j] = A[i, j]
   return out
 
 

@@ -185,6 +185,21 @@ class MsckfShape:
   def global_names(cls):
     return [f'g{i}' for i in range(cls.spec.get('n_globals', 0))]
 
+  @classmethod
+  def group(cls):
+    """Filters per group of the kernel that runs the plain kinds at EDIM <= 32 (pair kernel for even EDIM, single-warp
+    kernel for odd), as ``tests.shapes.ShapeFilter.group``."""
+    return 16 if cls.edim() % 2 == 0 else 14
+
+  @classmethod
+  def rts_kernel(cls):
+    """The smoother launch_rts_auto picks (main block only): 'mma' for even EDIM <= 32 with MEDIM >= 8, 'scalar' for
+    any other EDIM <= 32, None above (not built)."""
+    e = cls.edim()
+    if e > 32:
+      return None
+    return 'mma' if e % 2 == 0 and cls.medim() >= 8 else 'scalar'
+
 
 def batch(cls, B, seed=0):
   """Well-conditioned float64 inputs: x [B, DIM] (attitudes near the identity, so every clone sees the point ~20 units

@@ -2,7 +2,8 @@
 RaggedHistory) and is RTS-smoothed over its own rows and times (rts_smooth(RaggedHistory)).
 
 1. A lockstep stream recorded this way is bit-identical to step_recorded + rts_smooth(History) on every kernel path.
-2. Ragged streams at every tests/shapes.py shape, against the 40-digit reference of tests/hiprec.py.
+2. Ragged streams at every tests/shapes.py shape and at the MSCKF shapes with a smoother, against the 40-digit reference
+   of tests/hiprec.py.
 3. Live IMU + GNSS streams on per-filter clocks, against per-filter oracle driving and oracle/rts_numpy.
 4. A filter that outruns the history keeps stepping; the smoother refuses the history and says how many steps were lost.
 """
@@ -11,7 +12,8 @@ import pytest
 import torch
 
 from tests import hiprec
-from tests.shapes import SHAPES, batch, observe
+from tests.msckf_shapes import BY_NAME as MSCKF_BY_NAME, batch as msckf_batch, observe as msckf_observe
+from tests.shapes import SHAPES, batch as shape_batch, observe as shape_observe
 from tests.util import LIVE_R, Oracle, cov_err, kinematic_batch, live_batch, live_obs, state_err
 
 pytestmark = pytest.mark.gpu
@@ -30,7 +32,7 @@ def _dev(a):
 
 # ---------------------------------------------------------------------------------------------------- 1. lockstep ---
 def _lockstep_case(name):
-  """(folder, engine name, x, P, Q, quats, [(kind, z, R, ea)] per tick, smooth?) of one kernel path."""
+  """(folder, engine name, x, P, Q, quats, [(kind, z, R, ea)] per tick) of one kernel path."""
   from rednose_b200.filters import ensure_generated
   if name in ("live", "live_single"):
     from rednose_b200.filters.live import LiveKalman
@@ -40,38 +42,38 @@ def _lockstep_case(name):
       R = np.tile(np.diag(LIVE_R[kind]), (45, 1, 1))
       z = np.random.default_rng(k).normal(0, 0.05, (45, 3)) + (x[:, :3] if kind == 12 else [0, 0, -9.8] if kind == 10 else 0)
       ticks.append((kind, z, R, None))
-    return ensure_generated(LiveKalman), "live", x, P, Q, [3], ticks, True
+    return ensure_generated(LiveKalman), "live", x, P, Q, [3], ticks
   if name == "kinematic":
     from rednose_b200.filters.kinematic import KinematicKalman
     x, P, Q, z, R = kinematic_batch(300, seed=4)
     ticks = [(1, z + 0.01 * k, R, None) for k in range(5)]
-    return ensure_generated(KinematicKalman), "kinematic", x, P, Q, [], ticks, True
+    return ensure_generated(KinematicKalman), "kinematic", x, P, Q, [], ticks
   if name == "shape_e7":
     from tests.shapes import BY_NAME
     cls = BY_NAME[name]
     m = hiprec.model_of(cls)
     m.gv = [1.0 + 0.25 * i for i in range(len(m.gvars))]
-    x, P, Q, _ = batch(cls, 2 * cls.group() + 1, seed=5)
+    x, P, Q, _ = shape_batch(cls, 2 * cls.group() + 1, seed=5)
     kinds = [k for k, (_, _, g) in cls.kinds().items() if not g]
-    ticks = [(kinds[k % len(kinds)],) + observe(cls, m, kinds[k % len(kinds)], x, seed=k) for k in range(5)]
-    return ensure_generated(cls), cls.name, x, P, Q, cls.quat_idxs(), ticks, True
-  from tests.msckf_shapes import BY_NAME as MB, batch as mbatch, observe as mobserve
-  cls = MB["msckf_e18"]
+    ticks = [(kinds[k % len(kinds)],) + shape_observe(cls, m, kinds[k % len(kinds)], x, seed=k) for k in range(5)]
+    return ensure_generated(cls), cls.name, x, P, Q, cls.quat_idxs(), ticks
+  cls = MSCKF_BY_NAME[name]
   m = hiprec.model_of(cls)
-  x, P, Q, _ = mbatch(cls, 9, seed=6)
+  x, P, Q, _ = msckf_batch(cls, 9, seed=6)
   fk = cls.feature_kinds()[0]
-  ticks = [(fk,) + mobserve(cls, m, fk, x, seed=k) for k in range(3)]
-  return ensure_generated(cls), cls.name, x, P, Q, cls.quat_idxs(), ticks, False
+  plain = [k for k, v in cls.kinds().items() if not v[3]][0]
+  ticks = [(kind,) + msckf_observe(cls, m, kind, x, seed=k) for k, kind in enumerate([fk, plain, fk])]
+  return ensure_generated(cls), cls.name, x, P, Q, cls.quat_idxs(), ticks
 
 
-@pytest.mark.parametrize("case", ["live", "kinematic", "shape_e7", "live_single", "msckf_e18"])
+@pytest.mark.parametrize("case", ["live", "kinematic", "shape_e7", "live_single", "msckf_e18", "msckf_e28"])
 def test_lockstep_stream_equals_lockstep_recording_bit_for_bit(case, monkeypatch):
   """Every filter observes every tick with the same kind and time: RaggedScheduler(history=) + rts_smooth(ragged) ==
   step_recorded + rts_smooth(History), torch.equal on x, P, the four slabs and the smoothed rows."""
   from rednose_b200.scheduler import RaggedScheduler
   if case == "live_single":
     monkeypatch.setenv("REDNOSE_B200_WARP_KERNEL", "single")
-  folder, name, x, P, Q, q, ticks, smooth = _lockstep_case(case)
+  folder, name, x, P, Q, q, ticks = _lockstep_case(case)
   B, T = x.shape[0], len(ticks)
   a, b = _engine(folder, name, x, P, Q, q), _engine(folder, name, x, P, Q, q)
   h = a.new_history(T)
@@ -86,27 +88,32 @@ def test_lockstep_stream_equals_lockstep_recording_bit_for_bit(case, monkeypatch
   for s1, s2 in ((h.x_pred, rh.x_pred), (h.P_pred, rh.P_pred), (h.x_filt, rh.x_filt), (h.P_filt, rh.P_filt)):
     assert torch.equal(s1, s2)
   assert rh.n.tolist() == [T] * B and torch.equal(rh.t, h.t.new_tensor(h.t_host)[:, None].expand(T, B))
-  if smooth:
-    kw = dict(norm_quats=bool(q), quaternion_idxs=tuple(q) or (0,))
-    xs1, Ps1 = a.rts_smooth(h, **kw)
-    xs2, Ps2 = b.rts_smooth(rh, **kw)
-    assert torch.equal(xs1, xs2) and torch.equal(Ps1, Ps2)
+  kw = dict(norm_quats=bool(q), quaternion_idxs=tuple(q) or (0,))
+  xs1, Ps1 = a.rts_smooth(h, **kw)
+  xs2, Ps2 = b.rts_smooth(rh, **kw)
+  assert torch.equal(xs1, xs2) and torch.equal(Ps1, Ps2)
 
 
 # ------------------------------------------------------------------------------------------- 2. every shape, hiprec ---
-@pytest.mark.parametrize("cls", SHAPES, ids=[c.name for c in SHAPES])
+RAGGED_SHAPES = SHAPES + [MSCKF_BY_NAME[n] for n in ("msckf_e18", "msckf_e27", "msckf_e28")]
+
+
+@pytest.mark.parametrize("cls", RAGGED_SHAPES, ids=[c.name for c in RAGGED_SHAPES])
 def test_ragged_streams_against_the_40_digit_reference(cls):
   """B = 2G + 1 filters with 0 .. T recorded steps each, mixed kinds, irregular times, zero-dt pairs, one entry with two
   observations.  Final x / P of sampled filters against a per-filter 40-digit replay; their smoothed rows against
-  hiprec.rts over their own rows and times (with and without quaternion normalisation); rows past n[b] untouched."""
+  hiprec.rts over their own rows and times (with and without quaternion normalisation); rows past n[b] untouched.
+  An MSCKF (EDIM <= 32) also runs its gated feature kind on the CTA kernel and is smoothed on its main block."""
   from rednose_b200.filters import ensure_generated
+  msckf = cls in MSCKF_BY_NAME.values()
+  batch, observe = (msckf_batch, msckf_observe) if msckf else (shape_batch, shape_observe)
   G = cls.group()
   B, T = 2 * G + 1, 5
   m = hiprec.model_of(cls)
   m.gv = [1.0 + 0.25 * i for i in range(len(m.gvars))]
   x, P, Q, _ = batch(cls, B, seed=90)
   q = cls.quat_idxs()
-  kinds = [k for k, (_, _, g) in cls.kinds().items() if not g]
+  kinds = [k for k, v in cls.kinds().items() if not v[2] or (msckf and v[3])]
   rng = np.random.default_rng(91)
   mask = rng.random((B, T)) < 0.6
   mask[0] = False                       # no step at all
