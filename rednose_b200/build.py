@@ -27,21 +27,6 @@ def nvcc_path():
   return p
 
 
-TUNE_ENV = ("REDNOSE_B200_GROUP", "REDNOSE_B200_WARPS", "REDNOSE_B200_TMA", "REDNOSE_B200_STAGES", "REDNOSE_B200_TMA_STORE", "REDNOSE_B200_SMALLSYM",
-            "REDNOSE_B200_RTS_MMA", "REDNOSE_B200_MIN_WARPS", "REDNOSE_B200_PAIR", "REDNOSE_B200_PAIR_GROUP", "REDNOSE_B200_PAIR_MIN_WARPS",
-            "REDNOSE_B200_RTS_MIN_CTAS", "REDNOSE_B200_CTA_MIN_BLOCKS", "REDNOSE_B200_PAIR_WAR_FIX", "REDNOSE_B200_PAIR_LATE_REFILL", "REDNOSE_B200_MAXRREG")
-
-
-def _flags_match(folder, name):
-  """True if lib<name>.so in `folder` was built with the tuning flags the environment asks for now."""
-  want = " ".join(f"{e}={os.environ[e]}" for e in TUNE_ENV if os.environ.get(e))
-  try:
-    with open(os.path.join(folder, f".{name}.env"), encoding="utf-8") as f:
-      return f.read() == want
-  except OSError:
-    return want == ""
-
-
 def _newer(target, sources):
   if not os.path.exists(target):
     return False
@@ -58,27 +43,19 @@ def compile_filter(folder, name, force=False, verbose=False):
   """``{folder}/{name}.cu`` -> ``{folder}/lib{name}.so`` (sm_90a)."""
   src = os.path.join(folder, f"{name}.cu")
   lib = os.path.join(folder, f"lib{name}.so")
-  if not force and _newer(lib, [src] + csrc_sources()) and _flags_match(folder, name):
+  if not force and _newer(lib, [src] + csrc_sources()):
     return lib
   import fcntl
   with open(os.path.join(folder, f".{name}.lock"), "w") as lock:   # concurrent builders (one process per GPU) serialise here
     fcntl.flock(lock, fcntl.LOCK_EX)
-    if not force and _newer(lib, [src] + csrc_sources()) and _flags_match(folder, name):
+    if not force and _newer(lib, [src] + csrc_sources()):
       return lib
-    out = _compile_filter_locked(folder, name, src, lib, verbose)
-    with open(os.path.join(folder, f".{name}.env"), "w", encoding="utf-8") as f:
-      f.write(" ".join(f"{e}={os.environ[e]}" for e in TUNE_ENV if os.environ.get(e)))
-    return out
+    return _compile_filter_locked(folder, name, src, lib, verbose)
 
 
 def _compile_filter_locked(folder, name, src, lib, verbose):
-  tune = [f"-D{k}={os.environ[e]}" for k, e in (("RNB_GROUP", "REDNOSE_B200_GROUP"), ("RNB_WARPS", "REDNOSE_B200_WARPS"), ("RNB_TMA", "REDNOSE_B200_TMA"), ("RNB_STAGES", "REDNOSE_B200_STAGES"), ("RNB_TMA_STORE", "REDNOSE_B200_TMA_STORE"), ("RNB_SMALLSYM", "REDNOSE_B200_SMALLSYM"), ("RNB_RTS_MMA", "REDNOSE_B200_RTS_MMA"), ("RNB_MIN_WARPS", "REDNOSE_B200_MIN_WARPS"), ("RNB_PAIR", "REDNOSE_B200_PAIR"), ("RNB_PAIR_GROUP", "REDNOSE_B200_PAIR_GROUP"), ("RNB_PAIR_MIN_WARPS", "REDNOSE_B200_PAIR_MIN_WARPS"), ("RNB_RTS_MIN_CTAS", "REDNOSE_B200_RTS_MIN_CTAS"), ("RNB_CTA_MIN_BLOCKS", "REDNOSE_B200_CTA_MIN_BLOCKS"), ("RNB_PAIR_WAR_FIX", "REDNOSE_B200_PAIR_WAR_FIX"), ("RNB_PAIR_LATE_REFILL", "REDNOSE_B200_PAIR_LATE_REFILL")) if os.environ.get(e)]
-  if os.environ.get("REDNOSE_B200_MAXRREG"):
-    tune += ["-maxrregcount", os.environ["REDNOSE_B200_MAXRREG"]]
   tmp = lib + f".tmp{os.getpid()}"
-  cmd = [nvcc_path()] + NVCC_FLAGS + tune + ["-Xptxas", "-v", f"-I{CSRC_DIR}", f"-I{INCLUDE_DIR}", "-o", tmp, src]
-  with open(os.path.join(folder, f".{name}.flags"), "w", encoding="utf-8") as f:   # tuning flags this library was built with
-    f.write(" ".join(tune))
+  cmd = [nvcc_path()] + NVCC_FLAGS + ["-Xptxas", "-v", f"-I{CSRC_DIR}", f"-I{INCLUDE_DIR}", "-o", tmp, src]
   res = subprocess.run(cmd, capture_output=True, text=True)
   with open(os.path.join(folder, f"{name}.ptxas.log"), "w", encoding="utf-8") as f:
     f.write(" ".join(cmd) + "\n" + res.stdout + res.stderr)

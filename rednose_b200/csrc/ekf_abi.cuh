@@ -143,7 +143,7 @@ inline void launch_step(const StepArgs<M::NG>& a, cudaStream_t st) {
         last_status() = (int)cudaErrorMisalignedAddress;
         return;
       }
-      constexpr int G = RNB_PAIR_GROUP;
+      constexpr int G = PAIR_GROUP;
       const bool packed = a.flags & FLAG_PACKED_P;
       const size_t smem = packed ? pair_smem_bytes<M, K, G, true>() : pair_smem_bytes<M, K, G, false>();
       const unsigned grid = (unsigned)((a.B + G - 1) / G);
@@ -167,7 +167,7 @@ inline void launch_step(const StepArgs<M::NG>& a, cudaStream_t st) {
       }
     }
     if (!paired) {
-      constexpr int G = RNB_GROUP, W = RNB_WARPS;
+      constexpr int G = WARP_GROUP, W = WARP_CTA_WARPS;
       constexpr size_t smem = warp_smem_bytes<M, K, G, W>();
       const long long per_cta = (long long)G * W;
       const unsigned grid = (unsigned)((a.B + per_cta - 1) / per_cta);

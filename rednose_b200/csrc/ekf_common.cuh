@@ -73,7 +73,9 @@ __device__ __forceinline__ long long hist_slot(const StepArgs<NG>& a, long long 
 // The reference uses Eigen fullPivLu (ekf_c.c:89,101); S is symmetric positive
 // definite for any valid R, so an LDL^T factorisation (no square roots, Z
 // reciprocals) gives the same solution to rounding.  Everything is unrolled at
-// compile time so L/D live in registers.
+// compile time so L/D live in registers.  A closed-form adjugate inverse for
+// Z <= 3 was about 1 % faster but has about 10x the rounding error on
+// ill-conditioned S.
 // ---------------------------------------------------------------------------
 template <int Z>
 struct LDL {
@@ -114,60 +116,6 @@ struct LDL {
     }
   }
 };
-
-// Closed-form symmetric inverse for Z <= 3 (one reciprocal, cofactors computed independently: short dependency
-// chain), LDL^T otherwise.  Same interface as LDL: factor(S), solve(v).  S is SPD with modest condition number
-// (it is the innovation covariance H P H^T + R), so the adjugate is accurate to ~cond(S) * eps.
-template <int Z>
-struct SmallSym {
-  LDL<Z> ldl;
-  __device__ __forceinline__ void factor(const double (&S)[Z][Z]) { ldl.factor(S); }
-  __device__ __forceinline__ void solve(double (&v)[Z]) const { ldl.solve(v); }
-};
-template <>
-struct SmallSym<1> {
-  double i00;
-  __device__ __forceinline__ void factor(const double (&S)[1][1]) { i00 = 1.0 / S[0][0]; }
-  __device__ __forceinline__ void solve(double (&v)[1]) const { v[0] *= i00; }
-};
-template <>
-struct SmallSym<2> {
-  double i00, i01, i11;
-  __device__ __forceinline__ void factor(const double (&S)[2][2]) {
-    const double r = 1.0 / fma(S[0][0], S[1][1], -S[0][1] * S[0][1]);
-    i00 = S[1][1] * r; i01 = -S[0][1] * r; i11 = S[0][0] * r;
-  }
-  __device__ __forceinline__ void solve(double (&v)[2]) const {
-    const double a = v[0], b = v[1];
-    v[0] = fma(i00, a, i01 * b); v[1] = fma(i01, a, i11 * b);
-  }
-};
-template <>
-struct SmallSym<3> {
-  double i00, i01, i02, i11, i12, i22;
-  __device__ __forceinline__ void factor(const double (&S)[3][3]) {
-    const double a = S[0][0], b = S[0][1], c = S[0][2], d = S[1][1], e = S[1][2], f = S[2][2];
-    const double c00 = fma(d, f, -e * e), c01 = fma(c, e, -b * f), c02 = fma(b, e, -c * d);
-    const double c11 = fma(a, f, -c * c), c12 = fma(b, c, -a * e), c22 = fma(a, d, -b * b);
-    const double r = 1.0 / fma(a, c00, fma(b, c01, c * c02));
-    i00 = c00 * r; i01 = c01 * r; i02 = c02 * r; i11 = c11 * r; i12 = c12 * r; i22 = c22 * r;
-  }
-  __device__ __forceinline__ void solve(double (&v)[3]) const {
-    const double a = v[0], b = v[1], c = v[2];
-    v[0] = fma(i00, a, fma(i01, b, i02 * c));
-    v[1] = fma(i01, a, fma(i11, b, i12 * c));
-    v[2] = fma(i02, a, fma(i12, b, i22 * c));
-  }
-};
-
-#ifndef RNB_SMALLSYM
-#define RNB_SMALLSYM 0   // 1 = closed-form adjugate inverse for Z <= 3: ~1 % faster, ~10x larger rounding error on ill-conditioned S; off
-#endif
-#if RNB_SMALLSYM
-template <int Z> using SolverZ = SmallSym<Z>;
-#else
-template <int Z> using SolverZ = LDL<Z>;
-#endif
 
 // quaternion normalisation of x[idx..idx+4) -- division, like Eigen's normalize()
 __device__ __forceinline__ void normalize4(double* q) {

@@ -205,12 +205,10 @@ __device__ __forceinline__ void apply_reflectors(const double* V, const double* 
 
 template <class M>
 constexpr int cta_threads() { return ((M::EDIM + 31) / 32) * 32; }   // one thread per column
-#ifndef RNB_CTA_MIN_BLOCKS
-#define RNB_CTA_MIN_BLOCKS 4
-#endif
+constexpr int CTA_MIN_BLOCKS = 4;
 
 template <class M, class K, bool PRED, bool UPD, bool HIST = false>
-__global__ void __launch_bounds__(cta_threads<M>(), RNB_CTA_MIN_BLOCKS) ekf_step_cta(const StepArgs<M::NG> a, int o, const double* __restrict__ ws_all) {
+__global__ void __launch_bounds__(cta_threads<M>(), CTA_MIN_BLOCKS) ekf_step_cta(const StepArgs<M::NG> a, int o, const double* __restrict__ ws_all) {
   constexpr int D = M::DIM, E = M::EDIM, ME = M::MEDIM, Z = K::ZDIM, Y = K::YDIM, NR = Z - Y;
   using SM = CtaSmem<M, K>;
   using W = CtaWs<M, K>;

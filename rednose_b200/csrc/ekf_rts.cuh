@@ -68,10 +68,7 @@ __device__ __forceinline__ long long rts_rows(const RtsArgs<NG>& a, long long b)
 }
 
 constexpr int RTS_WARPS = 2;
-#ifndef RNB_RTS_MIN_CTAS
-#define RNB_RTS_MIN_CTAS 6
-#endif
-constexpr int RTS_MIN_CTAS = RNB_RTS_MIN_CTAS;
+constexpr int RTS_MIN_CTAS = 6;
 
 template <class M>
 struct RtsScratch {

@@ -21,13 +21,6 @@ __device__ __forceinline__ void dmma884(double& c0, double& c1, double a, double
   asm volatile("mma.sync.aligned.m8n8k4.row.col.f64.f64.f64.f64 {%0,%1}, {%2}, {%3}, {%0,%1};" : "+d"(c0), "+d"(c1) : "d"(a), "d"(b));
 }
 
-#ifndef RNB_RTS_PREFETCH
-#define RNB_RTS_PREFETCH 1   // pull the next step's history slabs into L2 while the current step computes
-#endif
-#ifndef RNB_RTS_PF_EARLY
-#define RNB_RTS_PF_EARLY 1   // P_{k|k} accumulator fragments loaded with the step's other global loads (one round trip)
-#endif
-
 __device__ __forceinline__ void prefetch_l2(const void* p) { asm volatile("prefetch.global.L2 [%0];" ::"l"(p)); }
 
 template <class M>
@@ -118,29 +111,26 @@ __global__ void __launch_bounds__(RTS_WARPS * 32, RTS_MIN_CTAS) ekf_rts_warp_mma
     // else -- inside the product loop each tile's load sat behind the previous tile's store to Ps (may alias) and
     // paid its own L2 round trip
     double pf[NT * NT * 2];
-    if constexpr (RNB_RTS_PF_EARLY) {
 #pragma unroll
-      for (int mi = 0; mi < NT; ++mi)
+    for (int mi = 0; mi < NT; ++mi)
 #pragma unroll
-        for (int ni = 0; ni < NT; ++ni) {
-          int r, c; frag_rc(mi, ni, r, c);
-          double2 v = make_double2(0.0, 0.0);
-          if (r < N && c < N) v = *reinterpret_cast<const double2*>(Pf_b + r * E + c);
-          pf[(mi * NT + ni) * 2] = v.x; pf[(mi * NT + ni) * 2 + 1] = v.y;
-        }
-    }
-    if constexpr (RNB_RTS_PREFETCH) {
-      if (k > 0) {   // step k-1 reads P_{k-1|k-1}, P_{k|k-1}, x_{k-1|k-1}, x_{k|k-1}: one 128-byte line per lane
-        constexpr int TB = E * E * (int)sizeof(double);
-        const int off = (lane * 128 < TB - 8) ? lane * 128 : TB - 8;
-        prefetch_l2(reinterpret_cast<const char*>(Pf_b - BP) + off);
-        prefetch_l2(reinterpret_cast<const char*>(a.hP_pred + k * BP + b * (long long)(E * E)) + off);
-        if (lane < 2) {
-          constexpr int XB = D * (int)sizeof(double);
-          const int xo = (lane * 128 < XB - 8) ? lane * 128 : XB - 8;
-          prefetch_l2(reinterpret_cast<const char*>(a.hx_filt + (k - 1) * BX + b * D) + xo);
-          prefetch_l2(reinterpret_cast<const char*>(a.hx_pred + k * BX + b * D) + xo);
-        }
+      for (int ni = 0; ni < NT; ++ni) {
+        int r, c; frag_rc(mi, ni, r, c);
+        double2 v = make_double2(0.0, 0.0);
+        if (r < N && c < N) v = *reinterpret_cast<const double2*>(Pf_b + r * E + c);
+        pf[(mi * NT + ni) * 2] = v.x; pf[(mi * NT + ni) * 2 + 1] = v.y;
+      }
+    // the next step's history slabs go into L2 while this step computes
+    if (k > 0) {   // step k-1 reads P_{k-1|k-1}, P_{k|k-1}, x_{k-1|k-1}, x_{k|k-1}: one 128-byte line per lane
+      constexpr int TB = E * E * (int)sizeof(double);
+      const int off = (lane * 128 < TB - 8) ? lane * 128 : TB - 8;
+      prefetch_l2(reinterpret_cast<const char*>(Pf_b - BP) + off);
+      prefetch_l2(reinterpret_cast<const char*>(a.hP_pred + k * BP + b * (long long)(E * E)) + off);
+      if (lane < 2) {
+        constexpr int XB = D * (int)sizeof(double);
+        const int xo = (lane * 128 < XB - 8) ? lane * 128 : XB - 8;
+        prefetch_l2(reinterpret_cast<const char*>(a.hx_filt + (k - 1) * BX + b * D) + xo);
+        prefetch_l2(reinterpret_cast<const char*>(a.hx_pred + k * BX + b * D) + xo);
       }
     }
     // dP = P_{k+1|N} - P_{k+1|k} in fragment layout -> shared memory (zero padded)
@@ -272,13 +262,7 @@ __global__ void __launch_bounds__(RTS_WARPS * 32, RTS_MIN_CTAS) ekf_rts_warp_mma
 #pragma unroll
       for (int mi = 0; mi < NT; ++mi) {
         int r, c; frag_rc(mi, ni, r, c);
-        double c0 = 0.0, c1 = 0.0;
-        if constexpr (RNB_RTS_PF_EARLY) {
-          c0 = pf[(mi * NT + ni) * 2]; c1 = pf[(mi * NT + ni) * 2 + 1];
-        } else if (r < N && c < N) {
-          const double2 t = *reinterpret_cast<const double2*>(Pf_b + r * E + c);
-          c0 = t.x; c1 = t.y;
-        }
+        double c0 = pf[(mi * NT + ni) * 2], c1 = pf[(mi * NT + ni) * 2 + 1];
 #pragma unroll
         for (int kq = 0; kq < NK; ++kq) dmma884(c0, c1, xb[kq][mi], yb[kq]);
         pn[(mi * NT + ni) * 2] = c0; pn[(mi * NT + ni) * 2 + 1] = c1;
@@ -297,10 +281,8 @@ __global__ void __launch_bounds__(RTS_WARPS * 32, RTS_MIN_CTAS) ekf_rts_warp_mma
   }
 }
 
-#ifndef RNB_RTS_MMA
-#define RNB_RTS_MMA 1   // 1: dense products of the smoother on the FP64 tensor path (DMMA); 0: scalar broadcast version
-#endif
-
+// dense products of the smoother on the FP64 tensor path (DMMA) where the fragment layout fits; the scalar broadcast
+// kernel otherwise
 template <class M>
 inline void launch_rts_auto(const RtsArgs<M::NG>& a, cudaStream_t st) {
   if (a.len && a.x_term) {
@@ -309,7 +291,7 @@ inline void launch_rts_auto(const RtsArgs<M::NG>& a, cudaStream_t st) {
     return;
   }
   if (a.B <= 0 || a.T <= 0) return;
-  if constexpr (RNB_RTS_MMA && M::EDIM <= 32 && M::EDIM % 2 == 0 && M::MEDIM >= 8) {
+  if constexpr (M::EDIM <= 32 && M::EDIM % 2 == 0 && M::MEDIM >= 8) {
     const unsigned grid = (unsigned)((a.B + RTS_WARPS - 1) / RTS_WARPS);
     constexpr size_t smem = sizeof(RtsMmaScratch<M>) * RTS_WARPS;   // 55 296 B at EDIM 32, 32 192 B for live_kf
     auto run = [&](void (*kern)(const RtsArgs<M::NG>)) {

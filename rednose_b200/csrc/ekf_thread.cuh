@@ -141,7 +141,7 @@ __global__ void __launch_bounds__(128) ekf_step_thread(const StepArgs<M::NG> a) 
         for (int j = 0; j < Z; ++j) S[i][j] = 0.0;
       K::S_accum(hv, [&](int c, int k) { return HP[c][k]; }, S);
 
-      SolverZ<Z> ldl;
+      LDL<Z> ldl;
       if constexpr (K::MAHA) {
         // ekf_c.c:88-94: gate = inflate R by 1e16 and still run the update
         double Sg[Z][Z];

@@ -33,32 +33,10 @@
 
 namespace rnb {
 
-// tuning knobs (overridable at build time: -DRNB_GROUP=..., -DRNB_WARPS=...)
-#ifndef RNB_GROUP
-#define RNB_GROUP 14  // filters per warp group (leaf phase uses RNB_GROUP of the 32 lanes)
-#endif
-#ifndef RNB_WARPS
-#define RNB_WARPS 1    // warps per CTA (warps never synchronise with each other)
-#endif
-
-#ifndef RNB_TMA
-#define RNB_TMA 1      // stage covariance tiles through shared memory with cp.async.bulk (TMA) load + store
-#endif
-#ifndef RNB_STAGES
-#define RNB_STAGES 1   // covariance tile ring per warp = bulk loads in flight per warp
-#endif
-#ifndef RNB_QDIAG_ASM
-#define RNB_QDIAG_ASM 1
-#endif
-#ifndef RNB_EX128
-#define RNB_EX128 1
-#endif
-#ifndef RNB_FV_EARLY
-#define RNB_FV_EARLY 0   // 1: F value slots are loaded before the tile wait -- measured: 74 more live registers, spills inside the per-filter loop
-#endif
-#ifndef RNB_TMA_STORE
-#define RNB_TMA_STORE 0  // 1: results leave through the tile with a bulk store; 0: plain coalesced stores from registers
-#endif
+constexpr int WARP_GROUP = 14;   // filters per warp group (leaf phase uses WARP_GROUP of the 32 lanes)
+constexpr int WARP_CTA_WARPS = 1;   // warps per CTA (warps never synchronise with each other)
+// covariance tile ring per warp = bulk loads in flight per warp; deeper rings cost occupancy and were slower
+constexpr int WARP_STAGES = 1;
 
 constexpr int even_up(int n) { return (n + 1) & ~1; }
 
@@ -81,11 +59,6 @@ __device__ __forceinline__ void tma_load_1d(void* smem_dst, const void* gsrc, ui
   asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
                ::"r"(smem_u32(smem_dst)), "l"(gsrc), "r"(bytes), "r"(smem_u32(bar)) : "memory");
 }
-__device__ __forceinline__ void tma_store_1d(void* gdst, const void* smem_src, uint32_t bytes) {
-  asm volatile("cp.async.bulk.global.shared::cta.bulk_group [%0], [%1], %2;" ::"l"(gdst), "r"(smem_u32(smem_src)), "r"(bytes) : "memory");
-  asm volatile("cp.async.bulk.commit_group;" ::: "memory");
-}
-__device__ __forceinline__ void tma_store_wait_read() { asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory"); }
 __device__ __forceinline__ void fence_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 
 // Per-filter row in shared memory.  Every section starts on an even index (16-byte aligned) so
@@ -125,12 +98,12 @@ __device__ __forceinline__ void vec_load(const double* src, double (&v)[N]) {
 }
 
 template <class M>
-constexpr bool use_tma() { return RNB_TMA && ((M::EDIM * M::EDIM) % 2 == 0); }  // bulk copies move multiples of 16 bytes
+constexpr bool use_tma() { return (M::EDIM * M::EDIM) % 2 == 0; }  // bulk copies move multiples of 16 bytes
 
 template <class M, class K, int G>
 struct WarpScratch {
   using L = RowLayout<M, K>;
-  static constexpr int NST = use_tma<M>() ? RNB_STAGES : 0;
+  static constexpr int NST = use_tma<M>() ? WARP_STAGES : 0;
   alignas(128) double tile[(NST > 0 ? NST : 1) * (use_tma<M>() ? M::EDIM * M::EDIM : 2)];  // covariance tiles (TMA ring)
   alignas(8) uint64_t full[NST > 0 ? NST : 1];                                              // "tile landed" mbarriers
   alignas(16) double rows[G * L::STRIDE];
@@ -205,12 +178,10 @@ __device__ __forceinline__ void scatter_out(double* __restrict__ g, const double
   }
 }
 
-#ifndef RNB_MIN_WARPS
-#define RNB_MIN_WARPS 12   // resident warps per SM the register allocator must allow (170 registers per thread)
-#endif
+constexpr int WARP_MIN_WARPS = 12;   // resident warps per SM the register allocator must allow (170 registers per thread)
 
 template <class M, class K, bool PRED, bool UPD, int G, int W, bool GATHER>
-__global__ void __launch_bounds__(W * 32, RNB_MIN_WARPS / W) ekf_step_warp(const StepArgs<M::NG> a) {
+__global__ void __launch_bounds__(W * 32, WARP_MIN_WARPS / W) ekf_step_warp(const StepArgs<M::NG> a) {
   constexpr int D = M::DIM, E = M::EDIM, Z = K::ZDIM;
   using L = RowLayout<M, K>;
   constexpr int RS = L::STRIDE;
@@ -247,7 +218,7 @@ __global__ void __launch_bounds__(W * 32, RNB_MIN_WARPS / W) ekf_step_warp(const
   auto hid_of = [&](int f) -> long long { return __shfl_sync(0xffffffffu, myhid, f); };   // gather lists only
 
   constexpr bool TMA = use_tma<M>();
-  constexpr int NST = TMA ? RNB_STAGES : 1;
+  constexpr int NST = TMA ? WARP_STAGES : 1;
   constexpr uint32_t TILE_BYTES = E * E * sizeof(double);
   uint32_t it = 0;  // tiles consumed so far by this warp (ring position / mbarrier parity)
   if constexpr (TMA) {
@@ -279,11 +250,8 @@ __global__ void __launch_bounds__(W * 32, RNB_MIN_WARPS / W) ekf_step_warp(const
         __syncwarp();
       }
       // prefetch the first covariance tiles of the group; they land while the leaf phase runs
-      if (lane == 0) {
-        if (RNB_TMA_STORE) tma_store_wait_read();  // (o > 0) tiles of the previous pass must have drained
-      }
 #pragma unroll
-      for (int k = 0; k < NST - (RNB_TMA_STORE ? 1 : 0); ++k) {
+      for (int k = 0; k < NST; ++k) {
         const long long fid = fid_of(k < ng ? k : 0);
         if (lane == 0 && k < ng) issue_load(fid, (it + k) % NST);
       }
@@ -388,9 +356,9 @@ __global__ void __launch_bounds__(W * 32, RNB_MIN_WARPS / W) ekf_step_warp(const
       double p[E];
       const uint32_t slot = it % NST;
       double* tile = s.tile + (TMA ? slot * (E * E) : 0);
-      // the F value slots do not depend on the tile: their (broadcast) loads go out before the wait
+      // the F value slots are loaded after the tile wait: loaded before it they held 74 more registers live and
+      // spilled inside the per-filter loop
       double fv[L::NFp];
-      if (RNB_FV_EARLY && do_pred) vec_load(row + L::OFF_FV, fv);
       if constexpr (TMA) {
         mbar_wait(&s.full[slot], (it / NST) & 1u);
         // P is symmetric: read ROW `lane` (contiguous, 128-bit accesses) as column `lane`
@@ -404,21 +372,12 @@ __global__ void __launch_bounds__(W * 32, RNB_MIN_WARPS / W) ekf_step_warp(const
 #pragma unroll
           for (int i = 0; i < E; ++i) p[i] = tile[i * E + col];
         }
-        if constexpr (RNB_TMA_STORE) {
-          // tile f+NST-1 goes into the slot whose store was issued one iteration ago
-          const long long nfid = fid_of(f + NST - 1 < ng ? f + NST - 1 : 0);
-          if (lane == 0 && f + NST - 1 < ng) {
-            tma_store_wait_read();
-            issue_load(nfid, (it + NST - 1) % NST);
-          }
-        } else {
-          // the slot is free as soon as every lane has its column in registers: refill it at once,
-          // keeping NST bulk loads in flight per warp
-          const long long nfid = fid_of(f + NST < ng ? f + NST : 0);
-          fence_async_smem();   // generic-proxy reads of the tile ordered before the async-proxy refill (see ekf_warp2.cuh)
-          __syncwarp();   // every lane has read its column before the slot is overwritten
-          if (lane == 0 && f + NST < ng) issue_load(nfid, slot);
-        }
+        // the slot is free as soon as every lane has its column in registers: refill it at once,
+        // keeping NST bulk loads in flight per warp
+        const long long nfid = fid_of(f + NST < ng ? f + NST : 0);
+        fence_async_smem();   // generic-proxy reads of the tile ordered before the async-proxy refill (see ekf_warp2.cuh)
+        __syncwarp();   // every lane has read its column before the slot is overwritten
+        if (lane == 0 && f + NST < ng) issue_load(nfid, slot);
       } else {
         const double* Pg = a.P + b * (long long)(E * E) + col;
 #pragma unroll
@@ -427,7 +386,7 @@ __global__ void __launch_bounds__(W * 32, RNB_MIN_WARPS / W) ekf_step_warp(const
       ++it;
 
       if (do_pred) {
-        if (!RNB_FV_EARLY) vec_load(row + L::OFF_FV, fv);
+        vec_load(row + L::OFF_FV, fv);
         const double dt = row[L::OFF_DT];
         // rows of F P that are not rows of P (F's non-identity rows) go through the exchange; every other
         // row j of F P equals column j of P (symmetry), which the lane already holds
@@ -444,17 +403,12 @@ __global__ void __launch_bounds__(W * 32, RNB_MIN_WARPS / W) ekf_step_warp(const
           const int slot_rf = __popc(M::FROW_MASK & ((1u << lane) - 1u));
           if (in_rf) {  // this lane's row of F P replaces its column of P
             const double* xr = s.exhp + slot_rf * EXS;
-            if constexpr (RNB_EX128) {
 #pragma unroll
-              for (int i = 0; i + 1 < E; i += 2) {
-                const double2 t = *reinterpret_cast<const double2*>(xr + i);
-                p[i] = t.x; p[i + 1] = t.y;
-              }
-              if constexpr (E % 2) p[E - 1] = xr[E - 1];
-            } else {
-#pragma unroll
-              for (int i = 0; i < E; ++i) p[i] = xr[i];
+            for (int i = 0; i + 1 < E; i += 2) {
+              const double2 t = *reinterpret_cast<const double2*>(xr + i);
+              p[i] = t.x; p[i + 1] = t.y;
             }
+            if constexpr (E % 2) p[E - 1] = xr[E - 1];
           }
           M::F_apply(fv, p);                        // column `lane` of F (F P)^T = F P F^T
           __syncwarp();
@@ -467,7 +421,6 @@ __global__ void __launch_bounds__(W * 32, RNB_MIN_WARPS / W) ekf_step_warp(const
           // one predicated DADD per element (a select costs ISETP + 2 FSEL + DADD; an `if` compiles to branches)
 #pragma unroll
           for (int i = 0; i < E; ++i)
-            if constexpr (!RNB_QDIAG_ASM) p[i] += (i == lane) ? dq : 0.0; else
             asm("{\n .reg .pred q;\n setp.eq.s32 q, %2, %3;\n @q add.f64 %0, %0, %1;\n}" : "+d"(p[i]) : "d"(dq), "r"(lane), "r"(i));
         } else {
           const double* Qg = a.Q + col;
@@ -502,7 +455,7 @@ __global__ void __launch_bounds__(W * 32, RNB_MIN_WARPS / W) ekf_step_warp(const
         vec_load(row + L::OFF_Y, y);
         vec_load(row + L::OFF_R, R);
 
-        SolverZ<Z> ldl;
+        LDL<Z> ldl;
         if constexpr (K::MAHA) {
           double Sg[Z][Z];
 #pragma unroll
@@ -556,15 +509,8 @@ __global__ void __launch_bounds__(W * 32, RNB_MIN_WARPS / W) ekf_step_warp(const
         }
       }
 
-      if constexpr (TMA && RNB_TMA_STORE) {
-        if (act) {
-#pragma unroll
-          for (int i = 0; i < E; ++i) tile[i * E + col] = p[i];
-        }
-        fence_async_smem();  // make the generic-proxy writes visible to the bulk-copy engine
-        __syncwarp();
-        if (lane == 0) tma_store_1d(a.P + b * (long long)(E * E), tile, TILE_BYTES);
-      } else if (act) {
+      // plain coalesced stores from registers: a bulk store of the tile was measured and was not faster
+      if (act) {
         double* Pg = a.P + b * (long long)(E * E) + col;
 #pragma unroll
         for (int i = 0; i < E; ++i) Pg[i * E] = p[i];
@@ -594,9 +540,6 @@ __global__ void __launch_bounds__(W * 32, RNB_MIN_WARPS / W) ekf_step_warp(const
       }
     }
     __syncwarp();
-  }
-  if constexpr (TMA && RNB_TMA_STORE) {
-    if (lane == 0) tma_store_wait_read();  // shared memory must outlive the bulk stores reading it
   }
 }
 

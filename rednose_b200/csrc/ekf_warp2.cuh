@@ -22,33 +22,14 @@
 
 namespace rnb {
 
-#ifndef RNB_PAIR
-#define RNB_PAIR 1        // 1: even-EDIM filters use ekf_step_pair; 0: always ekf_step_warp
-#endif
-#ifndef RNB_PAIR_GROUP
-#define RNB_PAIR_GROUP 16 // filters per warp group (leaf phase: one filter per lane)
-#endif
-#ifndef RNB_PAIR_MIN_WARPS
-#define RNB_PAIR_MIN_WARPS 8
-#endif
-#ifndef RNB_PAIR_FV_EARLY
-#define RNB_PAIR_FV_EARLY 0    // 1: F value slots are fetched before the tile wait instead of after it
-#endif
-#ifndef RNB_PAIR_WAR_FIX
-#define RNB_PAIR_WAR_FIX 1   // ordering of the tile reads before the slot refill: 1 = proxy fence (deterministic over 250 x 6.3e6 filter-steps), 2 = wait on the last load only (NOT sufficient: 66 of 250 runs differed), 3 = both
-#endif
-#ifndef RNB_PAIR_LATE_REFILL
-#define RNB_PAIR_LATE_REFILL 0   // 1: in fused-predict instantiations the fence + refill move behind the exchange stores of F P (the tile loads have long landed there)
-#endif
-#ifndef RNB_PAIR_TMA_STAGE
-#define RNB_PAIR_TMA_STAGE 1   // x / z / R / dt blocks of a full group arrive by bulk copy (one mbarrier wait, no registers held)
-#endif
+constexpr int PAIR_GROUP = 16;   // filters per warp group (leaf phase: one filter per lane)
+constexpr int PAIR_MIN_WARPS = 8;   // ~200 live values per lane: 255 registers, 8 one-warp CTAs per SM
 
 // Depth of the covariance tile ring (pairs in flight per warp).  A packed pair (live_kf: 4 224 B) is little more than half
 // a full one (7 744 B), so with the packed layout two slots cost about what one full slot does and the warp keeps two
-// pairs in flight at 8 warps per SM; the full layout (unflagged ABI, host_step) keeps RNB_STAGES slots of its size.
+// pairs in flight at 8 warps per SM; the full layout (unflagged ABI, host_step) keeps WARP_STAGES slots of its size.
 template <bool PACKED>
-constexpr int pair_stages() { return PACKED ? 2 : RNB_STAGES; }
+constexpr int pair_stages() { return PACKED ? 2 : WARP_STAGES; }
 
 template <class M, class K, int G, bool PACKED>
 struct PairScratch {
@@ -81,7 +62,7 @@ struct PairScratch {
 };
 
 template <class M, class K, bool PRED, bool UPD, int G, bool GATHER, bool PACKED>
-__global__ void __launch_bounds__(32, RNB_PAIR_MIN_WARPS) ekf_step_pair(const StepArgs<M::NG> a) {
+__global__ void __launch_bounds__(32, PAIR_MIN_WARPS) ekf_step_pair(const StepArgs<M::NG> a) {
   constexpr int D = M::DIM, E = M::EDIM, Z = K::ZDIM;
   using L = RowLayout<M, K>;
   using SC = PairScratch<M, K, G, PACKED>;
@@ -187,7 +168,7 @@ __global__ void __launch_bounds__(32, RNB_PAIR_MIN_WARPS) ekf_step_pair(const St
     // ---- stage x, z, R, dt of the group ----
     double dt_lane = a.dt;
     bool staged = false;
-    if constexpr (RNB_PAIR_TMA_STAGE && !GATHER) {
+    if constexpr (!GATHER) {
       // full group, 16-byte aligned arrays, one observation per filter: the blocks are contiguous -> bulk copies into
       // the (still idle) exchange buffers, one mbarrier wait; used at most once per kernel (o == 0), so parity 0
       const bool ok = o == 0 && ng == G && (!UPD || a.n_obs == 1) &&
@@ -320,8 +301,7 @@ __global__ void __launch_bounds__(32, RNB_PAIR_MIN_WARPS) ekf_step_pair(const St
       const uint32_t slot = it % NST;
       const double* tile = s.tile + slot * (2 * TS) + (valid ? h : 0) * TS;
       double p0[E], p1[E];                        // columns c0 and c0 + 1
-      double fv[L::NFp];
-      if (RNB_PAIR_FV_EARLY && do_pred) vec_load(row + L::OFF_FV, fv);
+      double fv[L::NFp];   // loaded after the tile wait: loaded before it, the F slots spill inside the loop
 
       mbar_wait(&s.full[slot], (it / NST) & 1u);
       // P is defined by its lower triangle.  Rows 2I, 2I+1 of the owned columns are the 2x2 block (I, hl) when I >= hl and
@@ -341,24 +321,18 @@ __global__ void __launch_bounds__(32, RNB_PAIR_MIN_WARPS) ekf_step_pair(const St
       }
       const int fn = f + 2 * NST;
       const long long fa = fid_of(fn < ng ? fn : 0), fb = fid_of(fn + 1 < ng ? fn + 1 : 0);
-      constexpr bool LATE = RNB_PAIR_LATE_REFILL && (M::NFROWS > 0);
-      if (!(LATE && do_pred)) {
-        // WAR across proxies: the 128-bit shared loads above are generic-proxy reads that may still be queued when this
-        // point is reached (a load is "issued", not "performed"); the bulk copy that refills the slot writes through the
-        // async proxy.  The proxy fence orders the reads before it -- without it about one filter-step in 1e7 saw the last
-        // tile rows of the NEXT pair (found as run-to-run differences of 10 000-step histories, scripts/dbg_rts_race.py).
-        if constexpr (RNB_PAIR_WAR_FIX & 1) fence_async_smem();
-        if constexpr (RNB_PAIR_WAR_FIX & 2) {   // experiment kept for the record: waiting on the LAST load of the sequence is NOT enough
-          const double landed = p0[E - 1] + p1[E - 1];
-          asm volatile("" ::"d"(landed));
-        }
-        __syncwarp();   // every lane holds its columns before the slot is refilled
-        if (lane == 0 && fn < ng) issue_pair(fn, slot, fa, fb);
-      }
+      // WAR across proxies: the 128-bit shared loads above are generic-proxy reads that may still be queued when this
+      // point is reached (a load is "issued", not "performed"); the bulk copy that refills the slot writes through the
+      // async proxy.  The proxy fence orders the reads before it -- without it about one filter-step in 1e7 saw the last
+      // tile rows of the NEXT pair (found as run-to-run differences of 10 000-step histories, scripts/dbg_rts_race.py).
+      // Waiting on the register of the last load instead is not sufficient (66 of 250 runs still differed).
+      fence_async_smem();
+      __syncwarp();   // every lane holds its columns before the slot is refilled
+      if (lane == 0 && fn < ng) issue_pair(fn, slot, fa, fb);
       ++it;
 
       if (do_pred) {
-        if (!RNB_PAIR_FV_EARLY) vec_load(row + L::OFF_FV, fv);
+        vec_load(row + L::OFF_FV, fv);
         const double dt = row[L::OFF_DT];
         if constexpr (M::NFROWS > 0) {
           {
@@ -379,9 +353,7 @@ __global__ void __launch_bounds__(32, RNB_PAIR_MIN_WARPS) ekf_step_pair(const St
               }
             }
           }
-          if constexpr (LATE) fence_async_smem();   // late refill: the tile loads landed long ago, the fence costs nothing here
           __syncwarp();
-          if constexpr (LATE) { if (lane == 0 && fn < ng) issue_pair(fn, slot, fa, fb); }
           // a column whose index is a non-identity row of F is replaced by that row of F P (symmetry gives the rest)
           if ((M::FROW_MASK >> c0) & 1u) {
             const double* xr = exh + SC::exrow(__popc(M::FROW_MASK & ((1u << c0) - 1u)));
@@ -446,7 +418,7 @@ __global__ void __launch_bounds__(32, RNB_PAIR_MIN_WARPS) ekf_step_pair(const St
         vec_load(row + L::OFF_Y, y);
         vec_load(row + L::OFF_R, R);
 
-        SolverZ<Z> ldl;
+        LDL<Z> ldl;
         if constexpr (K::MAHA) {
           double Sg[Z][Z];
 #pragma unroll
@@ -550,7 +522,7 @@ template <class M, class K, int G, bool PACKED>
 constexpr size_t pair_smem_bytes() { return sizeof(PairScratch<M, K, G, PACKED>); }
 
 template <class M>
-constexpr bool use_pair() { return RNB_PAIR && RNB_TMA && M::EDIM % 2 == 0 && M::EDIM <= 32; }
+constexpr bool use_pair() { return M::EDIM % 2 == 0 && M::EDIM <= 32; }
 
 // run-time escape hatch (and the way the tests reach ekf_step_warp on an even-EDIM filter):
 // REDNOSE_B200_WARP_KERNEL=single selects the one-filter-per-warp kernel; read at every launch (a getenv is

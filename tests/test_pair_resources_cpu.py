@@ -30,8 +30,8 @@ def compiled(tmp_path_factory):
     f'#include "{os.path.join(folder, "live.cu")}"\n'
     "#include <cstdio>\n"
     "template <class K> void show(int k) {\n"
-    "  printf(\"%d %zu %zu\\n\", k, rnb::pair_smem_bytes<live_model, K, RNB_PAIR_GROUP, true>(),\n"
-    "         rnb::pair_smem_bytes<live_model, K, RNB_PAIR_GROUP, false>());\n"
+    "  printf(\"%d %zu %zu\\n\", k, rnb::pair_smem_bytes<live_model, K, rnb::PAIR_GROUP, true>(),\n"
+    "         rnb::pair_smem_bytes<live_model, K, rnb::PAIR_GROUP, false>());\n"
     "}\n"
     "int main() {\n" + "".join(f"  show<live_kind_{k}>({k});\n" for k in LIVE_FUSED_KINDS) + "  return 0;\n}\n")
   exe = tmp / "sizes"
