@@ -26,6 +26,10 @@
  *     int <name>_packed_P_doubles(void)   doubles per filter of the packed layout, 0 where it is not used
  *     int <name>_convert_P(double *full, double *packed, const int *idx, long long n, int to_packed, void *stream)
  *         full [n, EDIM, EDIM] entry e <-> packed filter idx[e] (e when idx is NULL); returns the cudaError_t
+ *     int <name>_batch_rts_packed(...), <name>_batch_rts_segment_packed(...), <name>_batch_rts_ragged_packed(...)
+ *         the three smoothers with their arguments, over histories recorded with REDNOSE_PACKED_HIST: hP_pred, hP_filt,
+ *         the smoothed Ps (which may alias hP_filt) and P_term are packed; cudaErrorNotSupported where
+ *         <name>_packed_P_doubles() is 0
  *
  * All functions return void like the reference; CUDA failures are printed to stderr and
  * latched: `int <name>_cuda_status(void)` returns and clears the last cudaError_t (0 = ok).
@@ -48,6 +52,10 @@ extern "C" {
 /* P is [B, <name>_packed_P_doubles()] in the two-filters-per-warp kernel's packed lower-block-triangle layout
    (rednose_b200/csrc/ekf_packed.cuh); refused (cudaErrorNotSupported) wherever that kernel does not serve the launch */
 #define REDNOSE_PACKED_P 32
+/* hP_pred and hP_filt are [.., <name>_packed_P_doubles()] in the same layout (independent of REDNOSE_PACKED_P); refused
+   (cudaErrorNotSupported) wherever the two-filters-per-warp kernel does not serve the launch, and by host_step.  Such
+   histories are smoothed by <name>_batch_rts_packed / _rts_segment_packed / _rts_ragged_packed */
+#define REDNOSE_PACKED_HIST 64
 
 typedef void (*rednose_leaf3_fn)(double *, double *, double *);
 typedef void (*rednose_leaf2_fn)(double *, double *);

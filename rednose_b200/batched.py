@@ -12,6 +12,8 @@ Semantics follow the C++ driver: predict(dt) -> [normalise quaternions] -> updat
 Filters served by the two-filters-per-warp kernel (even EDIM <= 32, e.g. live_kf) keep P resident in that kernel's packed
 layout, the lower block triangle of 2x2 blocks (csrc/ekf_packed.cuh: 264 instead of 484 doubles per live filter), which
 halves the covariance traffic of a step.  ``P`` still reads as the full ``[B, EDIM, EDIM]`` tensor; see ``BatchedEKF.P``.
+For the same filters a history may record its covariances in that layout too (``new_history(T, packed=True)``), which
+shrinks a live history step from 8 112 to 4 592 bytes; ``unpack_P`` turns any packed slab back into full matrices.
 """
 from __future__ import annotations
 
@@ -26,6 +28,16 @@ Q_IS_DIAGONAL = 4
 SHARED_R = 8
 AUGMENT = 16   # fused clone-window shift (CTA kernel only)
 PACKED_P = 32  # P is in the packed lower-block-triangle layout (two-filters-per-warp kernel only)
+PACKED_HIST = 64  # the covariance history slabs are in that layout (same kernel only)
+
+PACKED_REFUSED = ("packed covariances exist only where the two-filters-per-warp kernel serves the filter (even EDIM <= 32, "
+                  "no feature-track kind, REDNOSE_B200_WARP_KERNEL != single)")
+
+
+def packed_P_doubles(folder, name):
+  """Doubles per filter of the packed covariance layout of filter `name` (csrc/ekf_packed.cuh), 0 where it is not used."""
+  _, lib = load_code(folder, name)
+  return int(getattr(lib, f"{name}_packed_P_doubles")())
 
 
 def _as_device(t, device, dtype=torch.float64):
@@ -154,6 +166,35 @@ class BatchedEKF:
   def _check(self, what):
     raise_on_cuda_error(self._lib, self.name, what)
 
+  def _hist_flag(self, *slabs):
+    """PACKED_HIST when the covariance history slabs (or rows of them) are packed [..., packed doubles], 0 when they are
+    full [..., EDIM, EDIM]; all of them must be in the same layout."""
+    packed = set()
+    for s in slabs:
+      if s is None:
+        continue
+      if tuple(s.shape[-2:]) == (self.dim_err, self.dim_err):
+        packed.add(False)
+      else:
+        assert self._packed_doubles and s.shape[-1] == self._packed_doubles, \
+          f"covariance history slab of shape {tuple(s.shape)}: neither [..., {self.dim_err}, {self.dim_err}] nor packed [..., {self._packed_doubles}]"
+        packed.add(True)
+    assert len(packed) <= 1, "the covariance history slabs of one launch must share one layout"
+    return PACKED_HIST if True in packed else 0
+
+  def unpack_P(self, packed):
+    """Full [..., EDIM, EDIM] covariances of packed ones [..., packed doubles] (a packed history slab, a row of one, or
+    the smoothed Ps of a packed history); a new tensor."""
+    assert self._packed_doubles and packed.shape[-1] == self._packed_doubles, (tuple(packed.shape), self._packed_doubles)
+    packed = packed.contiguous()
+    out = torch.empty(*packed.shape[:-1], self.dim_err, self.dim_err, dtype=torch.float64, device=packed.device)
+    n = packed.numel() // self._packed_doubles
+    if n:
+      with torch.cuda.device(self.device):
+        getattr(self._lib, f"{self.name}_convert_P")(self._p(out), self._p(packed), self._ffi.NULL, n, 0, self._stream())
+      self._check("convert_P")
+    return out
+
   def _dt_args(self, dt):
     if isinstance(dt, torch.Tensor):
       dt = dt.to(self.device, torch.float64).contiguous()
@@ -166,10 +207,11 @@ class BatchedEKF:
     """P <- F P F^T + dt Q, x <- f(x, dt) for the whole batch (ekf_c.c:8-33)."""
     keep, dt_ptr, dt_s = self._dt_args(dt)
     hx, hP = (hist if hist is not None else (None, None))
+    hflag = self._hist_flag(hP)
     P, pflag = self._P_arg()
     with torch.cuda.device(self.device):
       getattr(self._lib, f"{self.name}_batch_predict")(
-        self._p(self.x), P, self._cp(self.Q), dt_ptr, dt_s, self.B, self._quat, self._nquat, self.flags | pflag,
+        self._p(self.x), P, self._cp(self.Q), dt_ptr, dt_s, self.B, self._quat, self._nquat, self.flags | pflag | hflag,
         self._p(hx), self._p(hP), self._stream())
     self.launches += 1
     self._check("batch_predict")
@@ -195,11 +237,12 @@ class BatchedEKF:
     """Measurement update of one kind for the whole batch (ekf_c.c:37-121); returns the innovations y [B, n, m]."""
     z, R, ea, n_obs, flags = self._obs_args(z, R, ea)
     hx, hP = (hist if hist is not None else (None, None))
+    hflag = self._hist_flag(hP)
     P, pflag = self._P_arg()
     with torch.cuda.device(self.device):
       getattr(self._lib, f"{self.name}_batch_update_{kind}")(
         self._p(self.x), P, self._p(z), self._cp(R), self._cp(ea), n_obs, self.B,
-        self._quat, self._nquat, flags | pflag, self._p(hx), self._p(hP), self._stream())
+        self._quat, self._nquat, flags | pflag | hflag, self._p(hx), self._p(hP), self._stream())
     self.launches += 1
     self._check(f"batch_update_{kind}")
     return z
@@ -243,10 +286,12 @@ class BatchedEKF:
       else:
         assert t is not None, "a recorded step needs its time"
         assert hist.B == self.B, (hist.B, self.B)
+        hflag = self._hist_flag(hist.P_pred, hist.P_filt)
+        assert bool(hflag) == hist.packed
         rows = hist.reserve(idx, t)
         getattr(self._lib, f"{self.name}_batch_step_{kind}_hist_idx")(
           self._p(self.x), P, self._cp(self.Q), dt_ptr, dt_s, self._p(z), self._cp(R), self._cp(ea),
-          z.shape[1], n, self._quat, self._nquat, flags | pflag,
+          z.shape[1], n, self._quat, self._nquat, flags | pflag | hflag,
           self._p(hist.x_pred), self._p(hist.P_pred), self._p(hist.x_filt), self._p(hist.P_filt),
           idx_p, self._ffi.cast("const int *", rows.data_ptr()), hist.B, self._stream())
     self.launches += 1
@@ -264,11 +309,12 @@ class BatchedEKF:
       flags |= AUGMENT
     hxp, hPp = (hist_pred if hist_pred is not None else (None, None))
     hxf, hPf = (hist_filt if hist_filt is not None else (None, None))
+    hflag = self._hist_flag(hPp, hPf)
     P, pflag = self._P_arg()
     with torch.cuda.device(self.device):
       getattr(self._lib, f"{self.name}_batch_step_{kind}")(
         self._p(self.x), P, self._cp(self.Q), dt_ptr, dt_s, self._p(z), self._cp(R), self._cp(ea),
-        n_obs, self.B, self._quat, self._nquat, flags | pflag, self._p(hxp), self._p(hPp), self._p(hxf), self._p(hPf),
+        n_obs, self.B, self._quat, self._nquat, flags | pflag | hflag, self._p(hxp), self._p(hPp), self._p(hxf), self._p(hPf),
         self._stream())
     self.launches += 1
     self._check(f"batch_step_{kind}")
@@ -362,15 +408,25 @@ class BatchedEKF:
     self._check("batch_augment")
 
   # ------------------------------------------------------- history + smoothing ---
-  def new_history(self, T):
-    """Device slabs for a T-step history, time-major: what the reference keeps as the list of
-    9-tuples returned by predict_and_update_batch (ekf_sym.py:531): x_{k|k-1}, x_{k|k}, P_{k|k-1}, P_{k|k}, t."""
-    return History(T, self.B, self.dim_x, self.dim_err, self.device)
+  def _history_doubles(self, packed):
+    if not packed:
+      return 0
+    if not self._packed_doubles:
+      raise ValueError(f"filter '{self.name}': packed histories are not available: {PACKED_REFUSED}")
+    return self._packed_doubles
 
-  def new_ragged_history(self, T):
+  def new_history(self, T, packed=False):
+    """Device slabs for a T-step history, time-major: what the reference keeps as the list of
+    9-tuples returned by predict_and_update_batch (ekf_sym.py:531): x_{k|k-1}, x_{k|k}, P_{k|k-1}, P_{k|k}, t.
+
+    packed=True records the covariances in the packed layout of the resident P ([T, B, packed doubles]: 57 % of the
+    bytes of a live history step); raises ValueError where this filter has no packed layout."""
+    return History(T, self.B, self.dim_x, self.dim_err, self.device, self._history_doubles(packed))
+
+  def new_ragged_history(self, T, packed=False):
     """Device slabs for up to T recorded steps PER FILTER, each filter on its own clock (step_indexed(..., hist=)):
-    row k of filter b is the k-th step that filter recorded."""
-    return RaggedHistory(T, self.B, self.dim_x, self.dim_err, self.device)
+    row k of filter b is the k-th step that filter recorded.  packed: as in new_history."""
+    return RaggedHistory(T, self.B, self.dim_x, self.dim_err, self.device, self._history_doubles(packed))
 
   def step_recorded(self, hist, kind, t, z, R, ea=None):
     """predict_and_update_batch that also appends this step to `hist` (the kernel writes the slabs itself)."""
@@ -389,7 +445,9 @@ class BatchedEKF:
     """Batched RTS backward pass over a recorded history (ekf_sym.py:651-690, one launch for all filters).
 
     Returns (xs [T, B, DIM], Ps [T, B, EDIM, EDIM]) on the device.  `norm_quats` normalises the quaternion(s)
-    at `quaternion_idxs` the way the reference normalises its hard-coded slice 3:7.
+    at `quaternion_idxs` the way the reference normalises its hard-coded slice 3:7.  A packed history (new_history(T,
+    packed=True)) gives packed Ps [T, B, packed doubles] (see unpack_P), and `out` / `terminal` covariances are packed
+    like it.
 
     `terminal=(x [B, DIM], P [B, EDIM, EDIM])` smooths one SEGMENT of a longer history (steps k0 .. k0 + T - 2): the
     recursion starts from that smoothed estimate of step k0 + T - 1, whose history entry (the last one recorded) only
@@ -405,20 +463,24 @@ class BatchedEKF:
     assert T >= 1
     hist.sync_times()
     if out is not None:
-      xs, Ps = out                      # caller-provided [T, B, DIM] / [T, B, EDIM, EDIM] buffers
+      xs, Ps = out                      # caller-provided [T, B, DIM] / [T, B, EDIM, EDIM] (packed: [T, B, PD]) buffers
+      assert xs.shape[0] >= T and Ps.shape[0] >= T and xs.shape[1:] == hist.x_filt.shape[1:] and Ps.shape[1:] == hist.P_filt.shape[1:], \
+        ("out must match the history's layout", tuple(xs.shape), tuple(Ps.shape), tuple(hist.P_filt.shape))
     else:
       xs = hist.x_filt if in_place else torch.empty_like(hist.x_filt)
       Ps = hist.P_filt if in_place else torch.empty_like(hist.P_filt)
     qi = self._ffi.new("int[]", list(quaternion_idxs) or [0])
+    sfx = "_packed" if hist.packed else ""
     with torch.cuda.device(self.device):
       if terminal is None and not k0:
-        getattr(self._lib, f"{self.name}_batch_rts")(
+        getattr(self._lib, f"{self.name}_batch_rts{sfx}")(
           self._cp(hist.x_pred), self._cp(hist.P_pred), self._cp(hist.x_filt), self._cp(hist.P_filt), self._cp(hist.t), 0,
           self._p(xs), self._p(Ps), T, self.B, qi, len(quaternion_idxs) if norm_quats else 0, 1 if norm_quats else 0, self._stream())
       else:
         xt, Pt = terminal if terminal is not None else (None, None)   # the LAST segment of a history has k0 > 0 but no terminal
-        assert xt is None or (xt.is_contiguous() and Pt.is_contiguous() and xt.shape == (self.B, self.dim_x) and Pt.shape == (self.B, self.dim_err, self.dim_err))
-        getattr(self._lib, f"{self.name}_batch_rts_segment")(
+        assert xt is None or (xt.is_contiguous() and Pt.is_contiguous() and xt.shape == (self.B, self.dim_x) and Pt.shape == hist.P_filt.shape[1:]), \
+          "terminal=(x [B, DIM], P [B, EDIM, EDIM] or, for a packed history, [B, packed doubles])"
+        getattr(self._lib, f"{self.name}_batch_rts_segment{sfx}")(
           self._cp(hist.x_pred), self._cp(hist.P_pred), self._cp(hist.x_filt), self._cp(hist.P_filt), self._cp(hist.t), 0,
           self._p(xs), self._p(Ps), T, self.B, qi, len(quaternion_idxs) if norm_quats else 0, 1 if norm_quats else 0,
           self._cp(xt), self._cp(Pt), int(k0), self._stream())
@@ -443,7 +505,7 @@ class BatchedEKF:
       Ps = torch.full_like(hist.P_filt, float("nan"))
     qi = self._ffi.new("int[]", list(quaternion_idxs) or [0])
     with torch.cuda.device(self.device):
-      getattr(self._lib, f"{self.name}_batch_rts_ragged")(
+      getattr(self._lib, f"{self.name}_batch_rts_ragged{'_packed' if hist.packed else ''}")(
         self._cp(hist.x_pred), self._cp(hist.P_pred), self._cp(hist.x_filt), self._cp(hist.P_filt), self._cp(hist.t),
         self._ffi.cast("const int *", hist.n.data_ptr()), self._p(xs), self._p(Ps), hist.T, self.B, qi,
         len(quaternion_idxs) if norm_quats else 0, 1 if norm_quats else 0, self._stream())
@@ -469,16 +531,22 @@ class _PackedGraph:
     return getattr(self.graph, name)
 
 
-class History:
-  """Time-major device buffers of a forward pass, consumed by the RTS kernel."""
+def _cov_shape(dim_err, packed_doubles):
+  return (packed_doubles,) if packed_doubles else (dim_err, dim_err)
 
-  def __init__(self, T, B, dim_x, dim_err, device):
+
+class History:
+  """Time-major device buffers of a forward pass, consumed by the RTS kernel.  `packed`: the covariance slabs are
+  [T, B, packed_doubles] in the packed layout (BatchedEKF.new_history(T, packed=True)) instead of [T, B, EDIM, EDIM]."""
+
+  def __init__(self, T, B, dim_x, dim_err, device, packed_doubles=0):
     kw = dict(dtype=torch.float64, device=device)
     self.T, self.B, self.n = T, B, 0
+    self.packed = bool(packed_doubles)
     self.x_pred = torch.empty(T, B, dim_x, **kw)
     self.x_filt = torch.empty(T, B, dim_x, **kw)
-    self.P_pred = torch.empty(T, B, dim_err, dim_err, **kw)
-    self.P_filt = torch.empty(T, B, dim_err, dim_err, **kw)
+    self.P_pred = torch.empty(T, B, *_cov_shape(dim_err, packed_doubles), **kw)
+    self.P_filt = torch.empty(T, B, *_cov_shape(dim_err, packed_doubles), **kw)
     self.t = torch.zeros(T, **kw)
     self.t_host = np.zeros(T)          # step times are collected on the host and uploaded once, before the backward pass
     self._t_pinned = None
@@ -493,19 +561,20 @@ class History:
 class RaggedHistory:
   """Per-filter histories of a batch whose filters step on their own clocks (BatchedEKF.step_indexed with hist=).
 
-  Slabs are [T, B, ...] in the full covariance layout, like History, but row k of filter b is the k-th step THAT
-  filter recorded: `n [B]` (int32) counts the rows each filter has used and `t [T, B]` holds their times.  A step of a
-  filter whose T rows are used up is not recorded; `overflow` counts those steps.  All bookkeeping stays on the
-  device (no host synchronisation per tick)."""
+  Slabs are [T, B, ...] in the full covariance layout (or, with `packed`, the packed one), like History, but row k of
+  filter b is the k-th step THAT filter recorded: `n [B]` (int32) counts the rows each filter has used and `t [T, B]`
+  holds their times.  A step of a filter whose T rows are used up is not recorded; `overflow` counts those steps.  All
+  bookkeeping stays on the device (no host synchronisation per tick)."""
 
-  def __init__(self, T, B, dim_x, dim_err, device):
+  def __init__(self, T, B, dim_x, dim_err, device, packed_doubles=0):
     assert T >= 1
     kw = dict(dtype=torch.float64, device=device)
     self.T, self.B = int(T), int(B)
+    self.packed = bool(packed_doubles)
     self.x_pred = torch.empty(T, B, dim_x, **kw)
     self.x_filt = torch.empty(T, B, dim_x, **kw)
-    self.P_pred = torch.empty(T, B, dim_err, dim_err, **kw)
-    self.P_filt = torch.empty(T, B, dim_err, dim_err, **kw)
+    self.P_pred = torch.empty(T, B, *_cov_shape(dim_err, packed_doubles), **kw)
+    self.P_filt = torch.empty(T, B, *_cov_shape(dim_err, packed_doubles), **kw)
     self.t = torch.zeros(T, B, **kw)
     self.n = torch.zeros(B, dtype=torch.int32, device=device)
     self.overflow = torch.zeros((), dtype=torch.int64, device=device)

@@ -368,6 +368,13 @@ def gen_code(folder, name, f_sym, dt_sym, x_sym, obs_eqs, dim_x, dim_err, eskf_p
   brr = "const double *hx_pred, const double *hP_pred, const double *hx_filt, const double *hP_filt, const double *t, const int *len, double *xs, double *Ps, int T, long long B, const int *quat_idxs, int n_quat, int norm_quats, void *stream"
   hdr.append(f"int {name}_batch_rts_ragged({brr});")
   c.append(f'extern "C" int {name}_batch_rts_ragged({brr}) {{ return rnb::call_status([&] {{ rnb::batch_rts_ragged<{model}>(ctx_(), hx_pred, hP_pred, hx_filt, hP_filt, t, len, xs, Ps, T, B, quat_idxs, n_quat, norm_quats, stream); }}); }}\n')
+  # the three smoothers over packed histories (REDNOSE_PACKED_HIST): hP_pred, hP_filt, Ps and P_term are
+  # [.., <name>_packed_P_doubles()]; int results like the ragged ones, refused where the pair kernel does not record them
+  for suffix, args, call in (("rts", br, f"batch_rts<{model}, true>(ctx_(), hx_pred, hP_pred, hx_filt, hP_filt, t, t_per_filter, xs, Ps, T, B, quat_idxs, n_quat, norm_quats, stream)"),
+                             ("rts_segment", brs, f"batch_rts<{model}, true>(ctx_(), hx_pred, hP_pred, hx_filt, hP_filt, t, t_per_filter, xs, Ps, T, B, quat_idxs, n_quat, norm_quats, stream, x_term, P_term, k0)"),
+                             ("rts_ragged", brr, f"batch_rts_ragged<{model}, true>(ctx_(), hx_pred, hP_pred, hx_filt, hP_filt, t, len, xs, Ps, T, B, quat_idxs, n_quat, norm_quats, stream)")):
+    hdr.append(f"int {name}_batch_{suffix}_packed({args});")
+    c.append(f'extern "C" int {name}_batch_{suffix}_packed({args}) {{ return rnb::call_status([&] {{ rnb::{call}; }}); }}\n')
 
   if msckf:
     ba = "double *x, double *P, long long B, void *stream"

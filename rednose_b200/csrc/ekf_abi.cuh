@@ -15,6 +15,7 @@
 #include "ekf_augment.cuh"
 #include <cstring>
 #include <mutex>
+#include <type_traits>
 #include <unordered_set>
 
 namespace rnb {
@@ -87,8 +88,11 @@ constexpr int THREAD_MAX_EDIM = 6;
 // feature-track kind is never served whole by the pair kernel (its feature kinds run on the CTA kernel, which reads the
 // full layout), so its P stays full
 template <class M>
+constexpr bool pair_may_serve() { return M::EDIM > THREAD_MAX_EDIM && use_pair<M>() && !M::HAS_FEATURE_KIND; }
+
+template <class M>
 inline bool pair_serves() {
-  if constexpr (M::EDIM > THREAD_MAX_EDIM && use_pair<M>() && !M::HAS_FEATURE_KIND) return pair_enabled();
+  if constexpr (pair_may_serve<M>()) return pair_enabled();
   else return false;
 }
 
@@ -96,12 +100,13 @@ inline bool pair_serves() {
 template <class M>
 inline int packed_P_doubles() { return pair_serves<M>() ? packed_doubles(M::EDIM) : 0; }
 
-// FLAG_PACKED_P on a launch that the pair kernel would not run: rejected before any CUDA call
+// FLAG_PACKED_P or FLAG_PACKED_HIST on a launch that the pair kernel would not run: rejected before any CUDA call
 template <class M, bool FEATURE_KIND>
 inline bool check_packed_flag(int flags, const char* what) {
-  if (!(flags & FLAG_PACKED_P) || (!FEATURE_KIND && pair_serves<M>())) return true;
-  fprintf(stderr, "[rednose_b200] %s: the packed covariance layout exists only for the two-filters-per-warp kernel "
-                  "(even EDIM <= 32, no feature kinds, REDNOSE_B200_WARP_KERNEL != single)\n", what);
+  if (!(flags & (FLAG_PACKED_P | FLAG_PACKED_HIST)) || (!FEATURE_KIND && pair_serves<M>())) return true;
+  fprintf(stderr, "[rednose_b200] %s: the packed covariance layout (%s) exists only for the two-filters-per-warp kernel "
+                  "(even EDIM <= 32, no feature kinds, REDNOSE_B200_WARP_KERNEL != single)\n", what,
+          (flags & FLAG_PACKED_P) ? "P" : "history slabs");
   last_status() = (int)cudaErrorNotSupported;
   return false;
 }
@@ -144,7 +149,7 @@ inline void launch_step(const StepArgs<M::NG>& a, cudaStream_t st) {
         return;
       }
       constexpr int G = PAIR_GROUP;
-      const bool packed = a.flags & FLAG_PACKED_P;
+      const bool packed = a.flags & FLAG_PACKED_P, phist = a.flags & FLAG_PACKED_HIST;
       const size_t smem = packed ? pair_smem_bytes<M, K, G, true>() : pair_smem_bytes<M, K, G, false>();
       const unsigned grid = (unsigned)((a.B + G - 1) / G);
       auto run = [&](void (*kern)(const StepArgs<M::NG>)) {
@@ -154,8 +159,18 @@ inline void launch_step(const StepArgs<M::NG>& a, cudaStream_t st) {
         }
         kern<<<grid, 32, smem, st>>>(a);
       };
+      // the packed-history kernels (FLAG_PACKED_HIST) of gather list GA, for either layout of P; instantiated only for the
+      // filters the pair kernel may serve (check_packed_flag refused the flag for the others)
+      auto phist_kernel = [&](auto ga) -> void (*)(const StepArgs<M::NG>) {
+        constexpr bool GA = decltype(ga)::value;
+        using MH = PackedHist<M>;
+        if constexpr (pair_may_serve<M>())
+          return packed ? ekf_step_pair<MH, K, PRED, UPD, G, GA, true> : ekf_step_pair<MH, K, PRED, UPD, G, GA, false>;
+        else return nullptr;
+      };
       if constexpr (PRED && UPD) {
-        if (a.idx) run(packed ? ekf_step_pair<M, K, PRED, UPD, G, true, true> : ekf_step_pair<M, K, PRED, UPD, G, true, false>);
+        if (phist) run(a.idx ? phist_kernel(std::true_type{}) : phist_kernel(std::false_type{}));
+        else if (a.idx) run(packed ? ekf_step_pair<M, K, PRED, UPD, G, true, true> : ekf_step_pair<M, K, PRED, UPD, G, true, false>);
         else run(packed ? ekf_step_pair<M, K, PRED, UPD, G, false, true> : ekf_step_pair<M, K, PRED, UPD, G, false, false>);
       } else {
         if (a.idx) {
@@ -163,7 +178,8 @@ inline void launch_step(const StepArgs<M::NG>& a, cudaStream_t st) {
           last_status() = (int)cudaErrorNotSupported;
           return;
         }
-        run(packed ? ekf_step_pair<M, K, PRED, UPD, G, false, true> : ekf_step_pair<M, K, PRED, UPD, G, false, false>);
+        if (phist) run(phist_kernel(std::false_type{}));
+        else run(packed ? ekf_step_pair<M, K, PRED, UPD, G, false, true> : ekf_step_pair<M, K, PRED, UPD, G, false, false>);
       }
     }
     if (!paired) {
@@ -278,11 +294,19 @@ inline void batch_maha(HostCtx<M>& ctx, const double* x, const double* P, const 
   check(cudaFreeAsync(scratch, (cudaStream_t)stream), "cudaFreeAsync(maha scratch)");
 }
 
-template <class M>
+// PH: the covariance slabs (hP_pred, hP_filt, Ps and P_term) are packed; only where the pair kernel records them so
+template <class M, bool PH>
+inline bool check_packed_hist(const char* what) {
+  if constexpr (PH) return check_packed_flag<M, false>(FLAG_PACKED_HIST, what);
+  else return true;
+}
+
+template <class M, bool PH = false>
 inline void batch_rts(HostCtx<M>& ctx, const double* hx_pred, const double* hP_pred, const double* hx_filt, const double* hP_filt,
                       const double* t, int t_per_filter, double* xs, double* Ps, int T, long long B,
                       const int* quat_idxs, int n_quat, int norm_quats, void* stream,
                       const double* x_term = nullptr, const double* P_term = nullptr, long long k0 = 0) {
+  if (!check_packed_hist<M, PH>("batch_rts_packed")) return;
   if (!check_quat_idxs(quat_idxs, n_quat, M::DIM)) return;
   RtsArgs<M::NG> a;
   memset(&a, 0, sizeof(a));
@@ -292,14 +316,16 @@ inline void batch_rts(HostCtx<M>& ctx, const double* hx_pred, const double* hP_p
   a.n_quat = n_quat;
   for (int i = 0; i < n_quat; ++i) a.quat_idx[i] = quat_idxs[i];
   for (int i = 0; i < (M::NG > 0 ? M::NG : 1); ++i) a.gv[i] = ctx.gv.v[i];
-  launch_rts_auto<M>(a, (cudaStream_t)stream);
+  if constexpr (PH && !pair_may_serve<M>()) return;   // refused above
+  else launch_rts_auto<M, PH>(a, (cudaStream_t)stream);
 }
 
 // RTS over a ragged history: filter b smooths rows 0 .. len[b] - 1 of [T, B, ...] slabs with its own times t [T, B]
-template <class M>
+template <class M, bool PH = false>
 inline void batch_rts_ragged(HostCtx<M>& ctx, const double* hx_pred, const double* hP_pred, const double* hx_filt, const double* hP_filt,
                              const double* t, const int* len, double* xs, double* Ps, int T, long long B,
                              const int* quat_idxs, int n_quat, int norm_quats, void* stream) {
+  if (!check_packed_hist<M, PH>("batch_rts_ragged_packed")) return;
   if (M::EDIM > 32) {
     fprintf(stderr, "[rednose_b200] batched RTS for EDIM=%d > 32 is not built into this library\n", M::EDIM);
     last_status() = (int)cudaErrorNotSupported;
@@ -318,7 +344,8 @@ inline void batch_rts_ragged(HostCtx<M>& ctx, const double* hx_pred, const doubl
   a.n_quat = n_quat;
   for (int i = 0; i < n_quat; ++i) a.quat_idx[i] = quat_idxs[i];
   for (int i = 0; i < (M::NG > 0 ? M::NG : 1); ++i) a.gv[i] = ctx.gv.v[i];
-  launch_rts_auto<M>(a, (cudaStream_t)stream);
+  if constexpr (PH && !pair_may_serve<M>()) return;   // refused above
+  else launch_rts_auto<M, PH>(a, (cudaStream_t)stream);
 }
 
 // ------------------------------------------------------ covariance layout conversion ---
@@ -369,8 +396,8 @@ inline void host_step(HostCtx<M>& ctx, double* x, double* P, const double* Q, co
                       const int* quat_idxs, int n_quat, int flags) {
   constexpr int D = M::DIM, E = M::EDIM, Z = K::ZDIM, EA = K::EADIM;
   if (!check_quat_idxs(quat_idxs, n_quat, D)) return;   // before any stream, allocation or copy
-  if (flags & FLAG_PACKED_P) {
-    fprintf(stderr, "[rednose_b200] host_step: host buffers hold the full [B, EDIM, EDIM] covariance; FLAG_PACKED_P is not accepted\n");
+  if (flags & (FLAG_PACKED_P | FLAG_PACKED_HIST)) {
+    fprintf(stderr, "[rednose_b200] host_step: host buffers hold the full [B, EDIM, EDIM] covariance; FLAG_PACKED_P and FLAG_PACKED_HIST are not accepted\n");
     last_status() = (int)cudaErrorNotSupported;
     return;
   }

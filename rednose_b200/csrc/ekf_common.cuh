@@ -24,7 +24,22 @@ enum : int {
   FLAG_SHARED_R           = 8,  // R points at ONE [ZDIM, ZDIM] matrix used by every filter / observation
   FLAG_AUGMENT            = 16, // MSCKF: shift the clone window after the (last) update, in the same launch (ekf_sym.py:527-528 -> :365-391); CTA kernel only
   FLAG_PACKED_P           = 32, // P is [B, packed_doubles(EDIM)] in the packed lower-block-triangle layout (ekf_packed.cuh); pair kernel only
+  FLAG_PACKED_HIST        = 64, // hP_pred / hP_filt hold packed_doubles(EDIM) per filter in that layout; pair kernel only
 };
+
+// A filter model whose covariance HISTORY slabs are packed (FLAG_PACKED_HIST, ekf_packed.cuh).  The kernels that record
+// and smooth histories are instantiated with PackedHist<M> in place of M, so that the instantiations without packed
+// history keep their symbols and their machine code.
+template <class M>
+struct PackedHist : M {
+  static constexpr bool PACKED_HIST = true;
+};
+template <class M, class = void>
+struct PackedHistOf { static constexpr bool value = false; };
+template <class M>
+struct PackedHistOf<M, decltype(void(M::PACKED_HIST))> { static constexpr bool value = M::PACKED_HIST; };
+template <class M>
+constexpr bool packed_hist() { return PackedHistOf<M>::value; }
 
 // One argument block per launch, passed by value (lives in the kernel parameter
 // constant bank: every field is warp-uniform).  NG = number of global_vars.
@@ -49,9 +64,9 @@ struct StepArgs {
   int quat_idx[MAX_QUAT];
   // optional history slabs for the RTS smoother (ekf_sym.py:510,523): written when non-null
   double* hx_pred;       // [B, DIM]        x_{k|k-1}
-  double* hP_pred;       // [B, EDIM, EDIM] P_{k|k-1}
+  double* hP_pred;       // [B, EDIM, EDIM] P_{k|k-1}; [B, packed_doubles(EDIM)] with FLAG_PACKED_HIST
   double* hx_filt;       // [B, DIM]        x_{k|k}
-  double* hP_filt;       // [B, EDIM, EDIM] P_{k|k}
+  double* hP_filt;       // [B, EDIM, EDIM] P_{k|k}; [B, packed_doubles(EDIM)] with FLAG_PACKED_HIST
   double gv[NG > 0 ? NG : 1];
   // ragged histories (gather list only): entry e records at slab element hist_row[e] * hist_B + idx[e] instead of
   // idx[e]; a negative row steps without recording.  nullptr = the slabs are indexed by filter.  Kept behind the

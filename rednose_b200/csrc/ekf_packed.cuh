@@ -28,4 +28,13 @@ RNB_HD constexpr int packed_index(int i, int j) {
   return i >= j ? packed_block(i >> 1, j >> 1) + 2 * (i & 1) + (j & 1) : packed_block(j >> 1, i >> 1) + 2 * (j & 1) + (i & 1);
 }
 
+// the element (i, j) that double t of a packed E x E covariance holds; the upper corner of diagonal block I is (2I, 2I + 1)
+RNB_HD void packed_element(int E, int t, int& i, int& j) {
+  int I = 0;
+  while (I + 1 < E / 2 && packed_block(I + 1, 0) <= t) ++I;
+  const int w = t - packed_block(I, 0);
+  i = 2 * I + ((w >> 1) & 1);
+  j = 2 * (w >> 2) + (w & 1);
+}
+
 }  // namespace rnb

@@ -26,9 +26,12 @@
 #pragma once
 #include "ekf_common.cuh"
 #include "ekf_warp.cuh"
+#include "ekf_packed.cuh"
 
 namespace rnb {
 
+// Covariance slabs (hP_pred, hP_filt, Ps, P_term) are full [.., EDIM, EDIM] or, in the kernels' PH (packed history)
+// instantiations, [.., packed_doubles(EDIM)] in the layout of ekf_packed.cuh.
 template <int NG>
 struct RtsArgs {
   const double* hx_pred;  // [T, B, DIM]         x_{k|k-1}
@@ -67,6 +70,20 @@ __device__ __forceinline__ long long rts_rows(const RtsArgs<NG>& a, long long b)
   return n < 0 ? 0 : (n > a.T ? a.T : n);
 }
 
+// Elements (r, c), (r, c + 1), c even, of a packed covariance Pb, read the way the pair kernel reads its tiles: P is
+// defined by its lower triangle.  Below the block diagonal the pair is one 128-bit load of block (r / 2, c / 2); above it
+// it is the transposed pair, column r of block (c / 2, r / 2); on a diagonal block the upper element is its lower mirror.
+__device__ __forceinline__ double2 packed_pair(const double* Pb, int r, int c) {
+  const int R = r >> 1, C = c >> 1;
+  if (R > C) return *reinterpret_cast<const double2*>(Pb + packed_block(R, C) + 2 * (r & 1));
+  if (R < C) {
+    const double* q = Pb + packed_block(C, R) + (r & 1);
+    return make_double2(q[0], q[2]);
+  }
+  const double* q = Pb + packed_block(R, R);
+  return (r & 1) ? *reinterpret_cast<const double2*>(q + 2) : make_double2(q[0], q[2]);
+}
+
 constexpr int RTS_WARPS = 2;
 constexpr int RTS_MIN_CTAS = 6;
 
@@ -85,12 +102,16 @@ struct RtsScratch {
   alignas(16) double dinv[(N + 1) & ~1];              // 1 / D[k]
 };
 
+// M = PackedHist<model>: every covariance slab (hP_pred, hP_filt, Ps, P_term) is packed
 template <class M, bool RAGGED = false>
 __global__ void __launch_bounds__(RTS_WARPS * 32, RTS_MIN_CTAS) ekf_rts_warp(const RtsArgs<M::NG> a) {
   constexpr int D = M::DIM, E = M::EDIM, N = M::MEDIM, D1 = M::DMAIN;
+  constexpr bool PH = packed_hist<M>();
   using SC = RtsScratch<M>;
   constexpr int LD = SC::LD;
   static_assert(E <= 32, "warp-per-filter RTS needs EDIM <= 32");
+  static_assert(!PH || E % 2 == 0, "the packed layout needs an even EDIM");
+  constexpr int PS = PH ? packed_doubles(E) : E * E;   // doubles of one filter's covariance in the slabs
   __shared__ SC s_all[RTS_WARPS];
   const int lane = threadIdx.x & 31, wib = threadIdx.x >> 5;
   const long long b = (long long)blockIdx.x * RTS_WARPS + wib;
@@ -101,7 +122,7 @@ __global__ void __launch_bounds__(RTS_WARPS * 32, RTS_MIN_CTAS) ekf_rts_warp(con
   const bool act = lane < N;        // owns a column of the main block
   const bool actE = lane < E;       // owns a column of the full covariance
   const int col = actE ? lane : 0;
-  const long long BP = a.B * (long long)(E * E), BX = a.B * (long long)D;
+  const long long BP = a.B * (long long)PS, BX = a.B * (long long)D;
 
   auto normalize_xn = [&]() {
     for (int q = 0; q < a.n_quat; ++q) {
@@ -118,6 +139,13 @@ __global__ void __launch_bounds__(RTS_WARPS * 32, RTS_MIN_CTAS) ekf_rts_warp(con
   {
     const long long k = T - 1;
     const bool seg = a.x_term != nullptr;
+    if constexpr (PH) {
+      const double* Pg = seg ? a.P_term + b * (long long)PS : a.hP_pred + k * BP + b * (long long)PS;
+      double* Po = a.Ps + k * BP + b * (long long)PS;
+#pragma unroll
+      for (int i = 0; i < N; ++i) pn[i] = Pg[packed_index(i, col)];
+      if (!seg) for (int t = lane; t < PS; t += 32) Po[t] = Pg[t];
+    } else {
     const double* Pg = (seg ? a.P_term + b * (long long)(E * E) : a.hP_pred + k * BP + b * (long long)(E * E)) + col;
     double* Po = a.Ps + k * BP + b * (long long)(E * E) + col;
 #pragma unroll
@@ -125,6 +153,7 @@ __global__ void __launch_bounds__(RTS_WARPS * 32, RTS_MIN_CTAS) ekf_rts_warp(con
       const double v = Pg[i * E];
       if (i < N) pn[i] = v;
       if (actE && !seg) Po[i * E] = v;
+    }
     }
     for (int i = lane; i < D; i += 32) s.xn[i] = seg ? a.x_term[b * D + i] : a.hx_pred[k * BX + b * D + i];
     __syncwarp();
@@ -136,11 +165,15 @@ __global__ void __launch_bounds__(RTS_WARPS * 32, RTS_MIN_CTAS) ekf_rts_warp(con
 
 #pragma unroll 1
   for (long long k = T - 2; k >= 0; --k) {
-    const double* Pf_g = a.hP_filt + k * BP + b * (long long)(E * E) + col;
-    const double* Pp_g = a.hP_pred + (k + 1) * BP + b * (long long)(E * E) + col;
+    const double* Pf_b = a.hP_filt + k * BP + b * (long long)PS;
+    const double* Pp_b = a.hP_pred + (k + 1) * BP + b * (long long)PS;
+    const double* Pf_g = Pf_b + col;
+    const double* Pp_g = Pp_b + col;
+    // element i of the lane's column of a covariance: P is defined by its lower triangle
+    auto el = [&](const double* Pb, const double* Pg, int i) { return PH ? Pb[packed_index(i, col)] : Pg[i * E]; };
     double g[N];
 #pragma unroll
-    for (int i = 0; i < N; ++i) g[i] = Pf_g[i * E];
+    for (int i = 0; i < N; ++i) g[i] = el(Pf_b, Pf_g, i);
     for (int i = lane; i < D; i += 32) {
       s.xf[i] = a.hx_filt[k * BX + b * D + i];
       s.xp[i] = a.hx_pred[(k + 1) * BX + b * D + i];
@@ -159,7 +192,7 @@ __global__ void __launch_bounds__(RTS_WARPS * 32, RTS_MIN_CTAS) ekf_rts_warp(con
     // A = column of P_{k+1|k};  dP column = P_{k+1|N} - P_{k+1|k} (pn is dead afterwards)
     double A[N];
 #pragma unroll
-    for (int i = 0; i < N; ++i) A[i] = Pp_g[i * E];
+    for (int i = 0; i < N; ++i) A[i] = el(Pp_b, Pp_g, i);
     if (act) {
 #pragma unroll
       for (int i = 0; i < N; ++i) s.DP[i * LD + lane] = pn[i] - A[i];
@@ -248,7 +281,7 @@ __global__ void __launch_bounds__(RTS_WARPS * 32, RTS_MIN_CTAS) ekf_rts_warp(con
     __syncwarp();
     // out = P_{k|k}[:, lane] + sum_r X[r][:] y[r]
 #pragma unroll
-    for (int i = 0; i < N; ++i) pn[i] = Pf_g[i * E];
+    for (int i = 0; i < N; ++i) pn[i] = el(Pf_b, Pf_g, i);
 #pragma unroll 1
     for (int r = 0; r < N; ++r) {
       const double yr = s.LT[r * LD + (act ? lane : 0)];
@@ -260,23 +293,50 @@ __global__ void __launch_bounds__(RTS_WARPS * 32, RTS_MIN_CTAS) ekf_rts_warp(con
       }
     }
     // lanes / rows outside the main block keep P_{k|k} (only the main block is smoothed, ekf_sym.py:686)
+    if constexpr (PH) {
+      // packed: the lane writes the lower part of its column, i >= col, and an even column also the upper corner of its
+      // diagonal block, the mirror of element (col + 1, col)
+      if (actE) {
+        double* Po = a.Ps + k * BP + b * (long long)PS;
+#pragma unroll
+        for (int i = 0; i < E; ++i) {
+          if (i >= col) {
+            const double v = (act && i < N) ? pn[i < N ? i : 0] : Pf_b[packed_index(i, col)];
+            Po[packed_index(i, col)] = v;
+            if (i == col + 1 && !(col & 1)) Po[packed_block(col >> 1, col >> 1) + 1] = v;
+          }
+        }
+      }
+      __syncwarp();
+      // carry P_{k|N} as stored, by its lower triangle (see ekf_rts_warp_mma)
+      const double* Pk = a.Ps + k * BP + b * (long long)PS;
+#pragma unroll
+      for (int i = 0; i < N; ++i) pn[i] = Pk[packed_index(i, col)];
+    } else {
     if (actE) {
       const double* Pfull = a.hP_filt + k * BP + b * (long long)(E * E) + col;
       double* Po = a.Ps + k * BP + b * (long long)(E * E) + col;
 #pragma unroll
       for (int i = 0; i < E; ++i) Po[i * E] = (act && i < N) ? pn[i < N ? i : 0] : Pfull[i * E];
     }
+    }
     __syncwarp();
   }
 }
 
-template <class M>
+// PH: the covariance slabs are packed (only instantiated for an even EDIM <= 32)
+template <class M, bool PH = false>
 inline void launch_rts(const RtsArgs<M::NG>& a, cudaStream_t st) {
   if (a.B <= 0 || a.T <= 0) return;
   if constexpr (M::EDIM <= 32) {
     const unsigned grid = (unsigned)((a.B + RTS_WARPS - 1) / RTS_WARPS);
-    if (a.len) ekf_rts_warp<M, true><<<grid, RTS_WARPS * 32, 0, st>>>(a);
-    else ekf_rts_warp<M><<<grid, RTS_WARPS * 32, 0, st>>>(a);
+    if constexpr (PH) {
+      if (a.len) ekf_rts_warp<PackedHist<M>, true><<<grid, RTS_WARPS * 32, 0, st>>>(a);
+      else ekf_rts_warp<PackedHist<M>><<<grid, RTS_WARPS * 32, 0, st>>>(a);
+    } else {
+      if (a.len) ekf_rts_warp<M, true><<<grid, RTS_WARPS * 32, 0, st>>>(a);
+      else ekf_rts_warp<M><<<grid, RTS_WARPS * 32, 0, st>>>(a);
+    }
     check(cudaGetLastError(), "ekf_rts launch");
   } else {
     fprintf(stderr, "[rednose_b200] batched RTS for EDIM=%d > 32 is not built into this library\n", M::EDIM);

@@ -40,12 +40,16 @@ struct RtsMmaScratch {
   alignas(16) double dinv[(N + 1) & ~1];
 };
 
+// M = PackedHist<model>: every covariance slab is packed (ekf_packed.cuh); fragments are read with packed_pair and only
+// the lower blocks of Ps are written
 template <class M, bool RAGGED = false>
 __global__ void __launch_bounds__(RTS_WARPS * 32, RTS_MIN_CTAS) ekf_rts_warp_mma(const RtsArgs<M::NG> a) {
   constexpr int D = M::DIM, E = M::EDIM, N = M::MEDIM, D1 = M::DMAIN;
+  constexpr bool PH = packed_hist<M>();
   using SC = RtsMmaScratch<M>;
   constexpr int LD = SC::LD, NP = SC::NP, LP = SC::LP, NT = NP / 8, NK = NP / 4;
   static_assert(E <= 32 && E % 2 == 0, "fragment I/O needs an even EDIM <= 32");
+  constexpr int PS = PH ? packed_doubles(E) : E * E;   // doubles of one filter's covariance in the slabs
   // dynamic: from a main block of 25 (NP = 32) the RTS_WARPS scratch blocks pass the 48 KB static limit
   extern __shared__ __align__(16) unsigned char rts_smem_raw[];
   SC* s_all = reinterpret_cast<SC*>(rts_smem_raw);
@@ -58,7 +62,7 @@ __global__ void __launch_bounds__(RTS_WARPS * 32, RTS_MIN_CTAS) ekf_rts_warp_mma
   const bool act = lane < N, actE = lane < E;
   const int col = actE ? lane : 0;
   const int fg = lane >> 2, ft = lane & 3;   // fragment coordinates: row fg, k / column pair ft
-  const long long BP = a.B * (long long)(E * E), BX = a.B * (long long)D;
+  const long long BP = a.B * (long long)PS, BX = a.B * (long long)D;
 
   auto normalize_xn = [&]() {
     for (int q = 0; q < a.n_quat; ++q) {
@@ -71,22 +75,27 @@ __global__ void __launch_bounds__(RTS_WARPS * 32, RTS_MIN_CTAS) ekf_rts_warp_mma
   };
   // element pair (r, c), (r, c+1) of tile (mi, ni) in accumulator layout
   auto frag_rc = [&](int mi, int ni, int& r, int& c) { r = mi * 8 + fg; c = ni * 8 + 2 * ft; };
+  // elements (r, c), (r, c + 1) of the covariance at Pb
+  auto pair_at = [&](const double* Pb, int r, int c) {
+    if constexpr (PH) return packed_pair(Pb, r, c);
+    else return *reinterpret_cast<const double2*>(Pb + r * E + c);
+  };
 
   // ---- start: smoothed = predicted at T-1 (ekf_sym.py:658-659); carried in fragment layout ----
   double pn[NT * NT * 2];
   {
     const long long k = T - 1;
     const bool seg = a.x_term != nullptr;   // segment continuation: start from the smoothed estimate handed in
-    const double* Pg = seg ? a.P_term + b * (long long)(E * E) : a.hP_pred + k * BP + b * (long long)(E * E);
-    double* Po = a.Ps + k * BP + b * (long long)(E * E);
-    if (!seg) for (int idx = lane; idx < E * E; idx += 32) Po[idx] = Pg[idx];
+    const double* Pg = seg ? a.P_term + b * (long long)PS : a.hP_pred + k * BP + b * (long long)PS;
+    double* Po = a.Ps + k * BP + b * (long long)PS;
+    if (!seg) for (int idx = lane; idx < PS; idx += 32) Po[idx] = Pg[idx];
 #pragma unroll
     for (int mi = 0; mi < NT; ++mi)
 #pragma unroll
       for (int ni = 0; ni < NT; ++ni) {
         int r, c; frag_rc(mi, ni, r, c);
         double2 v = make_double2(0.0, 0.0);
-        if (r < N && c < N) v = *reinterpret_cast<const double2*>(Pg + r * E + c);
+        if (r < N && c < N) v = pair_at(Pg, r, c);
         pn[(mi * NT + ni) * 2] = v.x; pn[(mi * NT + ni) * 2 + 1] = v.y;
       }
     for (int i = lane; i < D; i += 32) s.xn[i] = seg ? a.x_term[b * D + i] : a.hx_pred[k * BX + b * D + i];
@@ -99,14 +108,17 @@ __global__ void __launch_bounds__(RTS_WARPS * 32, RTS_MIN_CTAS) ekf_rts_warp_mma
 
 #pragma unroll 1
   for (long long k = T - 2; k >= 0; --k) {
-    const double* Pf_b = a.hP_filt + k * BP + b * (long long)(E * E);
-    const double* Pp_b = a.hP_pred + (k + 1) * BP + b * (long long)(E * E);
+    const double* Pf_b = a.hP_filt + k * BP + b * (long long)PS;
+    const double* Pp_b = a.hP_pred + (k + 1) * BP + b * (long long)PS;
     const double* Pf_g = Pf_b + col;
     const double* Pp_g = Pp_b + col;
     // every global load of the step is issued here, before any dependent work (one latency round trip per step)
     double g[N], A[N];
 #pragma unroll
-    for (int i = 0; i < N; ++i) { g[i] = Pf_g[i * E]; A[i] = Pp_g[i * E]; }
+    for (int i = 0; i < N; ++i) {
+      if constexpr (PH) { g[i] = Pf_b[packed_index(i, col)]; A[i] = Pp_b[packed_index(i, col)]; }   // lower triangle
+      else { g[i] = Pf_g[i * E]; A[i] = Pp_g[i * E]; }
+    }
     // P_{k|k} once more, in accumulator layout (the C operand of the last product): fetched here with everything
     // else -- inside the product loop each tile's load sat behind the previous tile's store to Ps (may alias) and
     // paid its own L2 round trip
@@ -117,15 +129,15 @@ __global__ void __launch_bounds__(RTS_WARPS * 32, RTS_MIN_CTAS) ekf_rts_warp_mma
       for (int ni = 0; ni < NT; ++ni) {
         int r, c; frag_rc(mi, ni, r, c);
         double2 v = make_double2(0.0, 0.0);
-        if (r < N && c < N) v = *reinterpret_cast<const double2*>(Pf_b + r * E + c);
+        if (r < N && c < N) v = pair_at(Pf_b, r, c);
         pf[(mi * NT + ni) * 2] = v.x; pf[(mi * NT + ni) * 2 + 1] = v.y;
       }
     // the next step's history slabs go into L2 while this step computes
     if (k > 0) {   // step k-1 reads P_{k-1|k-1}, P_{k|k-1}, x_{k-1|k-1}, x_{k|k-1}: one 128-byte line per lane
-      constexpr int TB = E * E * (int)sizeof(double);
+      constexpr int TB = PS * (int)sizeof(double);
       const int off = (lane * 128 < TB - 8) ? lane * 128 : TB - 8;
       prefetch_l2(reinterpret_cast<const char*>(Pf_b - BP) + off);
-      prefetch_l2(reinterpret_cast<const char*>(a.hP_pred + k * BP + b * (long long)(E * E)) + off);
+      prefetch_l2(reinterpret_cast<const char*>(a.hP_pred + k * BP + b * (long long)PS) + off);
       if (lane < 2) {
         constexpr int XB = D * (int)sizeof(double);
         const int xo = (lane * 128 < XB - 8) ? lane * 128 : XB - 8;
@@ -141,7 +153,7 @@ __global__ void __launch_bounds__(RTS_WARPS * 32, RTS_MIN_CTAS) ekf_rts_warp_mma
         int r, c; frag_rc(mi, ni, r, c);
         double2 v = make_double2(0.0, 0.0);
         if (r < N && c < N) {
-          const double2 pp = *reinterpret_cast<const double2*>(Pp_b + r * E + c);
+          const double2 pp = pair_at(Pp_b, r, c);
           v.x = pn[(mi * NT + ni) * 2] - pp.x;
           v.y = pn[(mi * NT + ni) * 2 + 1] - pp.y;
         }
@@ -266,24 +278,52 @@ __global__ void __launch_bounds__(RTS_WARPS * 32, RTS_MIN_CTAS) ekf_rts_warp_mma
 #pragma unroll
         for (int kq = 0; kq < NK; ++kq) dmma884(c0, c1, xb[kq][mi], yb[kq]);
         pn[(mi * NT + ni) * 2] = c0; pn[(mi * NT + ni) * 2 + 1] = c1;
-        if (r < N && c < N) *reinterpret_cast<double2*>(a.Ps + k * BP + b * (long long)(E * E) + r * E + c) = make_double2(c0, c1);
+        if constexpr (PH) {
+          // lower blocks only: below the block diagonal one 128-bit store; on a diagonal block row r + 1 stores the
+          // block's lower row and, into the upper corner, the mirror of its element (r + 1, r); row r stores (r, r)
+          if (r < N && c < N && (r >> 1) >= (c >> 1)) {
+            double* q = a.Ps + k * BP + b * (long long)PS + packed_block(r >> 1, c >> 1);
+            if ((r >> 1) > (c >> 1) || (r & 1)) *reinterpret_cast<double2*>(q + 2 * (r & 1)) = make_double2(c0, c1);
+            else q[0] = c0;
+            if ((r >> 1) == (c >> 1) && (r & 1)) q[1] = c0;
+          }
+        } else {
+          if (r < N && c < N) *reinterpret_cast<double2*>(a.Ps + k * BP + b * (long long)(E * E) + r * E + c) = make_double2(c0, c1);
+        }
       }
     }
     // rows / columns outside the main block keep P_{k|k} (ekf_sym.py:686 smooths the main block only)
     if constexpr (E > N) {
-      double* Po = a.Ps + k * BP + b * (long long)(E * E);
-      for (int idx = lane; idx < E * E; idx += 32) {
-        const int i = idx / E, j = idx - i * E;
+      double* Po = a.Ps + k * BP + b * (long long)PS;
+      for (int idx = lane; idx < PS; idx += 32) {
+        int i, j;
+        if constexpr (PH) packed_element(E, idx, i, j);
+        else { i = idx / E; j = idx - i * E; }
         if (i >= N || j >= N) Po[idx] = Pf_b[idx];
       }
     }
     __syncwarp();
+    if constexpr (PH) {
+      // carry P_{k|N} as stored, by its lower triangle: the next step (or the segment smoothed after this one, from its
+      // terminal estimate) then starts from the same matrix, bit for bit
+      const double* Pk = a.Ps + k * BP + b * (long long)PS;
+#pragma unroll
+      for (int mi = 0; mi < NT; ++mi)
+#pragma unroll
+        for (int ni = 0; ni < NT; ++ni) {
+          int r, c; frag_rc(mi, ni, r, c);
+          if (r < N && c < N) {
+            const double2 v = packed_pair(Pk, r, c);
+            pn[(mi * NT + ni) * 2] = v.x; pn[(mi * NT + ni) * 2 + 1] = v.y;
+          }
+        }
+    }
   }
 }
 
 // dense products of the smoother on the FP64 tensor path (DMMA) where the fragment layout fits; the scalar broadcast
-// kernel otherwise
-template <class M>
+// kernel otherwise.  PH: the covariance slabs are packed (callers check that the pair kernel serves M)
+template <class M, bool PH = false>
 inline void launch_rts_auto(const RtsArgs<M::NG>& a, cudaStream_t st) {
   if (a.len && a.x_term) {
     fprintf(stderr, "[rednose_b200] RTS: per-filter lengths and segment continuation cannot be combined\n");
@@ -298,10 +338,14 @@ inline void launch_rts_auto(const RtsArgs<M::NG>& a, cudaStream_t st) {
       if (first_launch_of((const void*)kern)) cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
       kern<<<grid, RTS_WARPS * 32, smem, st>>>(a);
     };
-    run(a.len ? ekf_rts_warp_mma<M, true> : ekf_rts_warp_mma<M, false>);
+    if constexpr (PH) run(a.len ? ekf_rts_warp_mma<PackedHist<M>, true> : ekf_rts_warp_mma<PackedHist<M>, false>);
+    else run(a.len ? ekf_rts_warp_mma<M, true> : ekf_rts_warp_mma<M, false>);
     check(cudaGetLastError(), "ekf_rts_mma launch");
+  } else if constexpr (PH && !(M::EDIM <= 32 && M::EDIM % 2 == 0)) {
+    fprintf(stderr, "[rednose_b200] RTS: no packed covariance layout for EDIM = %d\n", M::EDIM);
+    last_status() = (int)cudaErrorNotSupported;
   } else {
-    launch_rts<M>(a, st);
+    launch_rts<M, PH>(a, st);
   }
 }
 

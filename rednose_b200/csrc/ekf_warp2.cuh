@@ -61,6 +61,12 @@ struct PairScratch {
   alignas(8) uint64_t stg;                            // "staging blocks landed" mbarrier
 };
 
+// doubles of one filter's entry in the history slabs hP_pred / hP_filt
+template <class M>
+constexpr int hist_doubles() { return packed_hist<M>() ? packed_doubles(M::EDIM) : M::EDIM * M::EDIM; }
+
+// M = PackedHist<model>: the history slabs hP_pred / hP_filt are packed (FLAG_PACKED_HIST).  (packed_hist<M>() and
+// hist_doubles<M>() are not held in local constants: such a local moves the register allocation of the other instantiations.)
 template <class M, class K, bool PRED, bool UPD, int G, bool GATHER, bool PACKED>
 __global__ void __launch_bounds__(32, PAIR_MIN_WARPS) ekf_step_pair(const StepArgs<M::NG> a) {
   constexpr int D = M::DIM, E = M::EDIM, Z = K::ZDIM;
@@ -146,6 +152,26 @@ __global__ void __launch_bounds__(32, PAIR_MIN_WARPS) ekf_step_pair(const StepAr
         *reinterpret_cast<double2*>(Pm + (c0 + 1) * E + 2 * I) = make_double2(q1[2 * I], q1[2 * I + 1]);
       }
     }
+  };
+  // packed layout (a.P with FLAG_PACKED_P, both history slabs with FLAG_PACKED_HIST): the lane's blocks (I, hl), I >= hl,
+  // one 32-byte block per iteration, two 128-bit stores.  For hP_pred this is the lower triangle of what store_cols writes.
+  auto store_packed = [&](double* Pg, const double (&q0)[E], const double (&q1)[E]) {
+#pragma unroll
+    for (int I = 0; I < E / 2; ++I) {
+      if (I >= hl) {
+        double* q = Pg + packed_block(I, hl);
+        *reinterpret_cast<double2*>(q) = make_double2(q0[2 * I], I == hl ? q0[2 * I + 1] : q1[2 * I]);
+        *reinterpret_cast<double2*>(q + 2) = make_double2(q0[2 * I + 1], q1[2 * I + 1]);
+      }
+    }
+  };
+  auto store_hpred = [&](double* Pm, const double (&q0)[E], const double (&q1)[E]) {
+    if constexpr (packed_hist<M>()) store_packed(Pm, q0, q1);
+    else store_cols(Pm, q0, q1);
+  };
+  auto store_hfilt = [&](double* Pm, const double (&q0)[E], const double (&q1)[E]) {
+    if constexpr (packed_hist<M>()) store_packed(Pm, q0, q1);
+    else store_full(Pm, q0, q1);
   };
 
   // diagonal process noise entries of the two owned columns
@@ -389,9 +415,9 @@ __global__ void __launch_bounds__(32, PAIR_MIN_WARPS) ekf_step_pair(const StepAr
         }
         if constexpr (GATHER) {
           const long long hb = hist_el();
-          if (a.hP_pred && wr && hb >= 0) store_cols(a.hP_pred + hb * (long long)(E * E), p0, p1);
+          if (a.hP_pred && wr && hb >= 0) store_hpred(a.hP_pred + hb * (long long)hist_doubles<M>(), p0, p1);
         }
-        else { if (a.hP_pred && wr) store_cols(a.hP_pred + b * (long long)(E * E), p0, p1); }
+        else { if (a.hP_pred && wr) store_hpred(a.hP_pred + b * (long long)hist_doubles<M>(), p0, p1); }
       }
 
       if constexpr (UPD) {
@@ -466,26 +492,17 @@ __global__ void __launch_bounds__(32, PAIR_MIN_WARPS) ekf_step_pair(const StepAr
           p0[i] = a0; p0[i + 1] = a1; p1[i] = b0v; p1[i + 1] = b1v;
         }
         __syncwarp();
-        if constexpr (!GATHER) { if (a.hP_filt && wr && o == n_obs - 1) store_full(a.hP_filt + b * (long long)(E * E), p0, p1); }   // = the state, bit for bit
+        if constexpr (!GATHER) { if (a.hP_filt && wr && o == n_obs - 1) store_hfilt(a.hP_filt + b * (long long)hist_doubles<M>(), p0, p1); }   // = the state, bit for bit
         else {
           const long long hb = hist_el();
-          if (a.hP_filt && wr && hb >= 0 && o == n_obs - 1) store_full(a.hP_filt + hb * (long long)(E * E), p0, p1);
+          if (a.hP_filt && wr && hb >= 0 && o == n_obs - 1) store_hfilt(a.hP_filt + hb * (long long)hist_doubles<M>(), p0, p1);
         }
       }
 
       const long long bp = GATHER ? fid_of(fi) : b;   // gather lists: shuffled again here rather than held through the update
       if (wr) {
         if constexpr (PACKED) {
-          // the lane's blocks (I, hl), I >= hl: one 32-byte block per iteration, two 128-bit stores
-          double* Pg = a.P + bp * (long long)TS;
-#pragma unroll
-          for (int I = 0; I < E / 2; ++I) {
-            if (I >= hl) {
-              double* q = Pg + packed_block(I, hl);
-              *reinterpret_cast<double2*>(q) = make_double2(p0[2 * I], I == hl ? p0[2 * I + 1] : p1[2 * I]);
-              *reinterpret_cast<double2*>(q + 2) = make_double2(p0[2 * I + 1], p1[2 * I + 1]);
-            }
-          }
+          store_packed(a.P + bp * (long long)TS, p0, p1);
         } else {
           store_full(a.P + bp * (long long)(E * E), p0, p1);
         }

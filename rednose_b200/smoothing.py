@@ -6,42 +6,69 @@ walks the list of tuples returned by predict_and_update_batch): 2*EDIM^2 + 2*DIM
 TILES of filters whose whole history fits the HBM budget; each tile runs forward-store-then-backward-consume and
 hands its smoothed track to a sink before the next tile reuses the buffers (SURVEY.md section 7, hard part 3).
 Tiles are independent, so multi-GPU use is: shard the filters over ranks first, tile within a rank.
+
+Both smoothers take ``packed_history=True`` for filters with a packed covariance layout (BatchedEKF.new_history(T,
+packed=True)): the history then stores each covariance as its packed lower block triangle (4 592 instead of 8 112 bytes
+per live filter-step, so 1.77x the filters per tile), and the sink receives the smoothed covariances packed,
+[..., packed doubles]; ``unpack_P`` turns them into full matrices.
 """
 from __future__ import annotations
 
 import torch
 
-from rednose_b200.batched import BatchedEKF
+from rednose_b200.batched import PACKED_REFUSED, BatchedEKF, packed_P_doubles
 
 
-def history_bytes_per_filter(dim_x, dim_err, T, smoothed_in_place=True):
-  per_step = 2 * dim_err * dim_err + 2 * dim_x
+def history_bytes_per_filter(dim_x, dim_err, T, smoothed_in_place=True, packed_doubles=0):
+  """Bytes of a T-step history of one filter; packed_doubles > 0: its covariances are in the packed layout of that many
+  doubles (BatchedEKF.new_history(T, packed=True))."""
+  cov = packed_doubles or dim_err * dim_err
+  per_step = 2 * cov + 2 * dim_x
   if not smoothed_in_place:
-    per_step += dim_err * dim_err + dim_x
+    per_step += cov + dim_x
   return 8 * per_step * T
 
 
+def _history_doubles(folder, name, packed_history):
+  if not packed_history:
+    return 0
+  pd = packed_P_doubles(folder, name)
+  if not pd:
+    raise ValueError(f"filter '{name}': packed histories are not available: {PACKED_REFUSED}")
+  return pd
+
+
 class TiledSmoother:
-  def __init__(self, folder, name, Q, dim_x, dim_err, quaternion_idxs=(), device="cuda", hbm_budget_bytes=60 << 30, tile=None):
+  """Forward filter + RTS smoother, one tile of filters with its whole history at a time.  With packed_history=True the
+  history and the smoothed covariances the sink receives are packed [T, n, packed doubles]; unpack_P(Ps) gives them full."""
+
+  def __init__(self, folder, name, Q, dim_x, dim_err, quaternion_idxs=(), device="cuda", hbm_budget_bytes=60 << 30, tile=None,
+               packed_history=False):
     self.folder, self.name, self.Q = folder, name, Q
     self.dim_x, self.dim_err = dim_x, dim_err
     self.quat = tuple(quaternion_idxs)
     self.device = torch.device(device)
     self.budget = hbm_budget_bytes
     self.tile = tile
+    self.packed_doubles = _history_doubles(folder, name, packed_history)
     self._engine = None
     self._hist = None
 
   def tile_size(self, T):
     if self.tile:
       return self.tile
-    per = history_bytes_per_filter(self.dim_x, self.dim_err, T) + 8 * (self.dim_err**2 + self.dim_x)
+    per = history_bytes_per_filter(self.dim_x, self.dim_err, T, packed_doubles=self.packed_doubles) + 8 * (self.dim_err**2 + self.dim_x)
     return max(1, int(self.budget // per))
+
+  def unpack_P(self, Ps):
+    """Full [..., EDIM, EDIM] covariances of packed smoothed ones (the sink's Ps with packed_history=True)."""
+    return self._engine.unpack_P(Ps)
 
   def run(self, x0, P0, T, obs_fn, sink, norm_quats=False, t0=0.0, passes=1):
     """x0 [B, DIM], P0 [B, EDIM, EDIM] (host or device).  obs_fn(k, lo, hi) -> (t, kind, z [hi-lo, m], R) gives the
-    observation of step k for filters lo..hi.  sink(lo, hi, xs [T, n, DIM], Ps [T, n, EDIM, EDIM]) receives device
-    views that are only valid during the call.  Returns the number of tiles.
+    observation of step k for filters lo..hi.  sink(lo, hi, xs [T, n, DIM], Ps [T, n, EDIM, EDIM], or [T, n, packed
+    doubles] with packed_history) receives device views that are only valid during the call.  Returns the number of
+    tiles.
 
     passes > 1: "multiple forward and backwards passes of the data" (reference README.md:41-45) -- each further pass
     restarts the forward filter of the tile from the previous pass's smoothed estimate at the first step
@@ -54,13 +81,13 @@ class TiledSmoother:
       n = hi - lo
       if self._engine is None or self._engine.B != n:
         self._engine = BatchedEKF(self.folder, self.name, self.Q, x0[lo:hi], P0[lo:hi], device=self.device, quaternion_idxs=self.quat)
-        self._hist = self._engine.new_history(T) if (self._hist is None or self._hist.B != n or self._hist.T != T) else self._hist
+        self._hist = self._engine.new_history(T, packed=bool(self.packed_doubles)) if (self._hist is None or self._hist.B != n or self._hist.T != T) else self._hist
       else:
         self._engine.init_state(x0[lo:hi], P0[lo:hi], None)
       eng, hist = self._engine, self._hist
       for p in range(max(1, int(passes))):
         if p > 0:   # the smoothed slabs alias the history buffers the next forward pass overwrites: copy step 0 out first
-          eng.init_state(xs[0].clone(), Ps[0].clone(), None)
+          eng.init_state(xs[0].clone(), eng.unpack_P(Ps[0]) if self.packed_doubles else Ps[0].clone(), None)
         hist.n = 0
         eng.filter_time = t0
         for k in range(T):
@@ -83,21 +110,30 @@ class CheckpointedSmoother:
   smoothed estimate handed over by that segment (`<name>_batch_rts_segment`).  Memory per filter is
   T / segment checkpoints + one segment of history instead of T steps of history, so ~100k live filters fit one tile;
   the price is a second forward pass.  The kernels are deterministic, so the result is bit-identical to smoothing the
-  whole history at once (tests/test_parity_gpu.py::test_checkpointed_smoother_equals_full_history)."""
+  whole history at once (tests/test_parity_gpu.py::test_checkpointed_smoother_equals_full_history).
 
-  def __init__(self, folder, name, Q, dim_x, dim_err, quaternion_idxs=(), device="cuda", hbm_budget_bytes=60 << 30, segment=64, tile=None):
+  packed_history=True: the segment history, the smoothed estimate handed between segments and the covariances the sink
+  receives are packed ([..., packed doubles]; unpack_P gives them full); the checkpoints stay full."""
+
+  def __init__(self, folder, name, Q, dim_x, dim_err, quaternion_idxs=(), device="cuda", hbm_budget_bytes=60 << 30, segment=64, tile=None,
+               packed_history=False):
     self.folder, self.name, self.Q = folder, name, Q
     self.dim_x, self.dim_err = dim_x, dim_err
     self.quat = tuple(quaternion_idxs)
     self.device = torch.device(device)
     self.budget, self.segment, self.tile = hbm_budget_bytes, int(segment), tile
+    self.packed_doubles = _history_doubles(folder, name, packed_history)
     self._engine = self._hist = self._ck = None
     self.stats = {}
 
   def bytes_per_filter(self, T):
     nseg = (T + self.segment - 1) // self.segment
     state = 8 * (self.dim_err**2 + self.dim_x)
-    return nseg * state + history_bytes_per_filter(self.dim_x, self.dim_err, self.segment + 1) + 3 * state
+    return nseg * state + history_bytes_per_filter(self.dim_x, self.dim_err, self.segment + 1, packed_doubles=self.packed_doubles) + 3 * state
+
+  def unpack_P(self, Ps):
+    """Full [..., EDIM, EDIM] covariances of packed smoothed ones (the sink's Ps with packed_history=True)."""
+    return self._engine.unpack_P(Ps)
 
   def tile_size(self, T):
     return self.tile or max(1, int(self.budget // self.bytes_per_filter(T)))
@@ -113,7 +149,7 @@ class CheckpointedSmoother:
     """obs_fn(k, lo, hi) -> (t, kind, z, R) must return the SAME observation every time it is asked for step k (each step
     is filtered twice) in a buffer the kernel may overwrite.  sink(lo, hi, k0, xs [n, tile, DIM], Ps [n, tile, EDIM, EDIM])
     receives the smoothed steps k0 .. k0 + n - 1 of filters lo..hi (segments arrive last to first; views valid during
-    the call only).  Returns the number of tiles."""
+    the call only; Ps [n, tile, packed doubles] with packed_history).  Returns the number of tiles."""
     B, S = x0.shape[0], self.segment
     n_tile, _ = self.plan(B, T)
     nseg = (T + S - 1) // S
@@ -126,11 +162,11 @@ class CheckpointedSmoother:
       if self._engine is None or self._engine.B != n:
         self._engine = self._hist = self._ck = self._term = None   # release the previous tile's buffers before allocating
         self._engine = BatchedEKF(self.folder, self.name, self.Q, x0[lo:hi], P0[lo:hi], device=self.device, quaternion_idxs=self.quat)
-        self._hist = self._engine.new_history(S + 1)
+        self._hist = self._engine.new_history(S + 1, packed=bool(self.packed_doubles))
         self._ck = (torch.empty(nseg, n, self.dim_x, dtype=torch.float64, device=self.device),
                     torch.empty(nseg, n, self.dim_err, self.dim_err, dtype=torch.float64, device=self.device))
         self._term = (torch.empty(n, self.dim_x, dtype=torch.float64, device=self.device),
-                      torch.empty(n, self.dim_err, self.dim_err, dtype=torch.float64, device=self.device))
+                      torch.empty(n, *self._hist.P_filt.shape[2:], dtype=torch.float64, device=self.device))
       else:
         self._engine.init_state(x0[lo:hi], P0[lo:hi], None)
       eng, hist, (ck_x, ck_P), (tx, tP) = self._engine, self._hist, self._ck, self._term
