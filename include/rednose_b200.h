@@ -15,7 +15,8 @@
  *     void <name>_set_<var>(double);                                                          ekf_sym.py:166-171
  *   batched additions, DEVICE pointers, B independent filters, AoS row-major float64
  *     void <name>_batch_predict(...), <name>_batch_update_<kind>(...), <name>_batch_step_<kind>(...)
- *     void <name>_batch_rts(...)   RTS smoother over a time-major history [T, B, ...]  (ekf_sym.py:651-690)
+ *     void <name>_batch_rts(...)   RTS smoother over a time-major history [T, B, ...]  (ekf_sym.py:651-690); an MSCKF is
+ *         smoothed on its main block, the rest of Ps is P_{k|k} (above EDIM 32 copied from hP_filt unless Ps is hP_filt)
  *   ragged histories (every filter records and smooths its own steps; int results = the call's cudaError_t):
  *     int <name>_batch_step_<kind>_hist_idx(...)   the gather step of <name>_batch_step_<kind>_idx; entry e also records at
  *         row hist_row[e] (negative: not recorded) of [T, hist_B, ...] history slabs

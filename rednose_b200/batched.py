@@ -428,14 +428,17 @@ class BatchedEKF:
     row k of filter b is the k-th step that filter recorded.  packed: as in new_history."""
     return RaggedHistory(T, self.B, self.dim_x, self.dim_err, self.device, self._history_doubles(packed))
 
-  def step_recorded(self, hist, kind, t, z, R, ea=None):
-    """predict_and_update_batch that also appends this step to `hist` (the kernel writes the slabs itself)."""
+  def step_recorded(self, hist, kind, t, z, R, ea=None, augment=False):
+    """predict_and_update_batch that also appends this step to `hist` (the kernel writes the slabs itself).  augment=True
+    shifts the MSCKF clone window after the update, as step(augment=True); the recorded x_{k|k} / P_{k|k} are the
+    estimate before the shift, as predict_and_update_batch(augment=True) returns it (ekf_sym.py:522-530)."""
     k = hist.n
     assert k < hist.T, "history is full"
     if self.filter_time is None:
       self.filter_time = t
     dt = t - self.filter_time
-    y = self.step(kind, dt, z, R, ea, hist_pred=(hist.x_pred[k], hist.P_pred[k]), hist_filt=(hist.x_filt[k], hist.P_filt[k]))
+    y = self.step(kind, dt, z, R, ea, hist_pred=(hist.x_pred[k], hist.P_pred[k]), hist_filt=(hist.x_filt[k], hist.P_filt[k]),
+                  augment=augment)
     self.filter_time = t
     hist.t_host[k] = float(t)
     hist.n += 1

@@ -317,7 +317,17 @@ inline void batch_rts(HostCtx<M>& ctx, const double* hx_pred, const double* hP_p
   for (int i = 0; i < n_quat; ++i) a.quat_idx[i] = quat_idxs[i];
   for (int i = 0; i < (M::NG > 0 ? M::NG : 1); ++i) a.gv[i] = ctx.gv.v[i];
   if constexpr (PH && !pair_may_serve<M>()) return;   // refused above
-  else launch_rts_auto<M, PH>(a, (cudaStream_t)stream);
+  else {
+    if constexpr (M::EDIM > 32) {
+      // above 32 the kernels write only the main block of Ps[0 .. T-2]; everything else there is P_{k|k}: nothing to do in
+      // place, one copy of those rows of hP_filt otherwise (row T-1 the kernel writes in full, or not at all for a segment)
+      if (B > 0 && T >= 2 && Ps != hP_filt &&
+          !check(cudaMemcpyAsync(Ps, hP_filt, sizeof(double) * (size_t)(T - 1) * (size_t)B * M::EDIM * M::EDIM,
+                                 cudaMemcpyDeviceToDevice, (cudaStream_t)stream), "cudaMemcpyAsync(RTS P_{k|k})"))
+        return;
+    }
+    launch_rts_auto<M, PH>(a, (cudaStream_t)stream);
+  }
 }
 
 // RTS over a ragged history: filter b smooths rows 0 .. len[b] - 1 of [T, B, ...] slabs with its own times t [T, B]

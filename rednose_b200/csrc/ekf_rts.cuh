@@ -1,4 +1,4 @@
-// rednose_b200 -- batched Rauch-Tung-Striebel backward pass (warp-per-filter, MEDIM <= EDIM <= 32).
+// rednose_b200 -- batched Rauch-Tung-Striebel backward pass (warp-per-filter, MEDIM <= 32).
 //
 // Reference: EKF_sym.rts_smooth, rednose/helpers/ekf_sym.py:651-690 (Python + numpy, one filter).  Per
 // filter the recursion over the stored history is strictly sequential, so one warp walks one filter's
@@ -23,6 +23,11 @@
 //   C dP C^T = X^T (dP X):  two dense n x n x n products with one operand broadcast from shared memory.
 // The smoothed covariance P_{k+1|N} is carried in registers between steps; per step the kernel
 // reads P_{k+1|k}, P_{k|k} and writes P_{k|N}: 3 EDIM^2 + 3 DIM doubles (SURVEY.md section 8d).
+//
+// Above EDIM 32 (an MSCKF, whose main block is at most 32 wide) a lane cannot own a column of the full covariance: lanes
+// < MEDIM read and write only the main block (row stride EDIM), other lanes load no covariance, and the rest of Ps[k] is
+// P_{k|k} before the launch (in place, or copied there by batch_rts): 3 MEDIM^2 + 3 DIM doubles per step.  Only whole and
+// segment histories in the full layout are smoothed there.
 #pragma once
 #include "ekf_common.cuh"
 #include "ekf_warp.cuh"
@@ -109,7 +114,8 @@ __global__ void __launch_bounds__(RTS_WARPS * 32, RTS_MIN_CTAS) ekf_rts_warp(con
   constexpr bool PH = packed_hist<M>();
   using SC = RtsScratch<M>;
   constexpr int LD = SC::LD;
-  static_assert(E <= 32, "warp-per-filter RTS needs EDIM <= 32");
+  static_assert(N <= 32, "warp-per-filter RTS needs MEDIM <= 32");
+  static_assert(E <= 32 || (!PH && !RAGGED), "above EDIM 32 only whole and segment histories in the full layout");
   static_assert(!PH || E % 2 == 0, "the packed layout needs an even EDIM");
   constexpr int PS = PH ? packed_doubles(E) : E * E;   // doubles of one filter's covariance in the slabs
   __shared__ SC s_all[RTS_WARPS];
@@ -145,6 +151,12 @@ __global__ void __launch_bounds__(RTS_WARPS * 32, RTS_MIN_CTAS) ekf_rts_warp(con
 #pragma unroll
       for (int i = 0; i < N; ++i) pn[i] = Pg[packed_index(i, col)];
       if (!seg) for (int t = lane; t < PS; t += 32) Po[t] = Pg[t];
+    } else if constexpr (E > 32) {
+      const double* Pg = seg ? a.P_term + b * (long long)(E * E) : a.hP_pred + k * BP + b * (long long)(E * E);
+      double* Po = a.Ps + k * BP + b * (long long)(E * E);
+#pragma unroll
+      for (int i = 0; i < N; ++i) pn[i] = act ? Pg[i * E + lane] : 0.0;
+      if (!seg) for (int t = lane; t < E * E; t += 32) Po[t] = Pg[t];
     } else {
     const double* Pg = (seg ? a.P_term + b * (long long)(E * E) : a.hP_pred + k * BP + b * (long long)(E * E)) + col;
     double* Po = a.Ps + k * BP + b * (long long)(E * E) + col;
@@ -170,7 +182,10 @@ __global__ void __launch_bounds__(RTS_WARPS * 32, RTS_MIN_CTAS) ekf_rts_warp(con
     const double* Pf_g = Pf_b + col;
     const double* Pp_g = Pp_b + col;
     // element i of the lane's column of a covariance: P is defined by its lower triangle
-    auto el = [&](const double* Pb, const double* Pg, int i) { return PH ? Pb[packed_index(i, col)] : Pg[i * E]; };
+    auto el = [&](const double* Pb, const double* Pg, int i) {
+      if constexpr (E > 32) return act ? Pg[i * E] : 0.0;   // main block only
+      else return PH ? Pb[packed_index(i, col)] : Pg[i * E];
+    };
     double g[N];
 #pragma unroll
     for (int i = 0; i < N; ++i) g[i] = el(Pf_b, Pf_g, i);
@@ -312,6 +327,12 @@ __global__ void __launch_bounds__(RTS_WARPS * 32, RTS_MIN_CTAS) ekf_rts_warp(con
       const double* Pk = a.Ps + k * BP + b * (long long)PS;
 #pragma unroll
       for (int i = 0; i < N; ++i) pn[i] = Pk[packed_index(i, col)];
+    } else if constexpr (E > 32) {
+      if (act) {
+        double* Po = a.Ps + k * BP + b * (long long)(E * E) + lane;
+#pragma unroll
+        for (int i = 0; i < N; ++i) Po[i * E] = pn[i];
+      }
     } else {
     if (actE) {
       const double* Pfull = a.hP_filt + k * BP + b * (long long)(E * E) + col;
@@ -324,11 +345,15 @@ __global__ void __launch_bounds__(RTS_WARPS * 32, RTS_MIN_CTAS) ekf_rts_warp(con
   }
 }
 
-// PH: the covariance slabs are packed (only instantiated for an even EDIM <= 32)
+// PH: the covariance slabs are packed (only instantiated for an even EDIM <= 32).  Above EDIM 32 the rest of Ps outside
+// the main block must already hold P_{k|k} (batch_rts), and ragged histories are refused by their caller.
 template <class M, bool PH = false>
 inline void launch_rts(const RtsArgs<M::NG>& a, cudaStream_t st) {
   if (a.B <= 0 || a.T <= 0) return;
-  if constexpr (M::EDIM <= 32) {
+  if constexpr (M::EDIM > 32 && M::MEDIM <= 32 && !PH) {
+    ekf_rts_warp<M><<<(unsigned)((a.B + RTS_WARPS - 1) / RTS_WARPS), RTS_WARPS * 32, 0, st>>>(a);
+    check(cudaGetLastError(), "ekf_rts launch");
+  } else if constexpr (M::EDIM <= 32) {
     const unsigned grid = (unsigned)((a.B + RTS_WARPS - 1) / RTS_WARPS);
     if constexpr (PH) {
       if (a.len) ekf_rts_warp<PackedHist<M>, true><<<grid, RTS_WARPS * 32, 0, st>>>(a);
@@ -339,7 +364,7 @@ inline void launch_rts(const RtsArgs<M::NG>& a, cudaStream_t st) {
     }
     check(cudaGetLastError(), "ekf_rts launch");
   } else {
-    fprintf(stderr, "[rednose_b200] batched RTS for EDIM=%d > 32 is not built into this library\n", M::EDIM);
+    fprintf(stderr, "[rednose_b200] batched RTS for EDIM=%d, MEDIM=%d is not built into this library\n", M::EDIM, M::MEDIM);
     last_status() = (int)cudaErrorNotSupported;
   }
 }

@@ -11,7 +11,8 @@
 //     loaded from / stored to global memory in (aligned 128-bit accesses).
 //
 // n is padded to a multiple of 8 with zeros (22 -> 24 for live_kf).  FP64 mma is IEEE fused multiply-add, so
-// results agree with the scalar kernel to rounding (different summation order).
+// results agree with the scalar kernel to rounding (different summation order).  Above EDIM 32 (an MSCKF) only the main
+// block of the slabs is read and written, as in ekf_rts_warp.
 #pragma once
 #include "ekf_rts.cuh"
 
@@ -48,7 +49,8 @@ __global__ void __launch_bounds__(RTS_WARPS * 32, RTS_MIN_CTAS) ekf_rts_warp_mma
   constexpr bool PH = packed_hist<M>();
   using SC = RtsMmaScratch<M>;
   constexpr int LD = SC::LD, NP = SC::NP, LP = SC::LP, NT = NP / 8, NK = NP / 4;
-  static_assert(E <= 32 && E % 2 == 0, "fragment I/O needs an even EDIM <= 32");
+  static_assert(E % 2 == 0 && N <= 32, "fragment I/O needs an even EDIM and MEDIM <= 32");
+  static_assert(E <= 32 || (!PH && !RAGGED), "above EDIM 32 only whole and segment histories in the full layout");
   constexpr int PS = PH ? packed_doubles(E) : E * E;   // doubles of one filter's covariance in the slabs
   // dynamic: from a main block of 25 (NP = 32) the RTS_WARPS scratch blocks pass the 48 KB static limit
   extern __shared__ __align__(16) unsigned char rts_smem_raw[];
@@ -117,6 +119,7 @@ __global__ void __launch_bounds__(RTS_WARPS * 32, RTS_MIN_CTAS) ekf_rts_warp_mma
 #pragma unroll
     for (int i = 0; i < N; ++i) {
       if constexpr (PH) { g[i] = Pf_b[packed_index(i, col)]; A[i] = Pp_b[packed_index(i, col)]; }   // lower triangle
+      else if constexpr (E > 32) { g[i] = act ? Pf_g[i * E] : 0.0; A[i] = act ? Pp_g[i * E] : 0.0; }   // main block only
       else { g[i] = Pf_g[i * E]; A[i] = Pp_g[i * E]; }
     }
     // P_{k|k} once more, in accumulator layout (the C operand of the last product): fetched here with everything
@@ -133,7 +136,22 @@ __global__ void __launch_bounds__(RTS_WARPS * 32, RTS_MIN_CTAS) ekf_rts_warp_mma
         pf[(mi * NT + ni) * 2] = v.x; pf[(mi * NT + ni) * 2 + 1] = v.y;
       }
     // the next step's history slabs go into L2 while this step computes
-    if (k > 0) {   // step k-1 reads P_{k-1|k-1}, P_{k|k-1}, x_{k-1|k-1}, x_{k|k-1}: one 128-byte line per lane
+    if constexpr (E > 32) {   // the main block's rows: lane r touches every 128-byte line of row r (points <= 16 doubles apart)
+      auto prefetch_row = [&](const double* r) {
+#pragma unroll
+        for (int o = 0; o < N; o += 16) prefetch_l2(r + o);
+        prefetch_l2(r + N - 1);
+      };
+      if (k > 0 && act) {
+        prefetch_row(Pf_b - BP + lane * E);
+        prefetch_row(a.hP_pred + k * BP + b * (long long)PS + lane * E);
+      }
+      if (k > 0 && lane < (D - 1) / 16 + 2) {   // x rows likewise: points at most 16 doubles apart, the last one included
+        const int xo = lane * 16 < D ? lane * 16 : D - 1;
+        prefetch_l2(a.hx_filt + (k - 1) * BX + b * D + xo);
+        prefetch_l2(a.hx_pred + k * BX + b * D + xo);
+      }
+    } else if (k > 0) {   // step k-1 reads P_{k-1|k-1}, P_{k|k-1}, x_{k-1|k-1}, x_{k|k-1}: one 128-byte line per lane
       constexpr int TB = PS * (int)sizeof(double);
       const int off = (lane * 128 < TB - 8) ? lane * 128 : TB - 8;
       prefetch_l2(reinterpret_cast<const char*>(Pf_b - BP) + off);
@@ -293,7 +311,7 @@ __global__ void __launch_bounds__(RTS_WARPS * 32, RTS_MIN_CTAS) ekf_rts_warp_mma
       }
     }
     // rows / columns outside the main block keep P_{k|k} (ekf_sym.py:686 smooths the main block only)
-    if constexpr (E > N) {
+    if constexpr (E > N && E <= 32) {   // above 32 batch_rts leaves P_{k|k} there before the launch
       double* Po = a.Ps + k * BP + b * (long long)PS;
       for (int idx = lane; idx < PS; idx += 32) {
         int i, j;
@@ -331,14 +349,15 @@ inline void launch_rts_auto(const RtsArgs<M::NG>& a, cudaStream_t st) {
     return;
   }
   if (a.B <= 0 || a.T <= 0) return;
-  if constexpr (M::EDIM <= 32 && M::EDIM % 2 == 0 && M::MEDIM >= 8) {
+  if constexpr (M::EDIM % 2 == 0 && M::MEDIM >= 8 && M::MEDIM <= 32 && (M::EDIM <= 32 || !PH)) {
     const unsigned grid = (unsigned)((a.B + RTS_WARPS - 1) / RTS_WARPS);
     constexpr size_t smem = sizeof(RtsMmaScratch<M>) * RTS_WARPS;   // 55 296 B at EDIM 32, 32 192 B for live_kf
     auto run = [&](void (*kern)(const RtsArgs<M::NG>)) {
       if (first_launch_of((const void*)kern)) cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
       kern<<<grid, RTS_WARPS * 32, smem, st>>>(a);
     };
-    if constexpr (PH) run(a.len ? ekf_rts_warp_mma<PackedHist<M>, true> : ekf_rts_warp_mma<PackedHist<M>, false>);
+    if constexpr (M::EDIM > 32) run(ekf_rts_warp_mma<M, false>);   // ragged histories are refused above 32 by their caller
+    else if constexpr (PH) run(a.len ? ekf_rts_warp_mma<PackedHist<M>, true> : ekf_rts_warp_mma<PackedHist<M>, false>);
     else run(a.len ? ekf_rts_warp_mma<M, true> : ekf_rts_warp_mma<M, false>);
     check(cudaGetLastError(), "ekf_rts_mma launch");
   } else if constexpr (PH && !(M::EDIM <= 32 && M::EDIM % 2 == 0)) {
