@@ -31,7 +31,7 @@ PACKED_P = 32  # P is in the packed lower-block-triangle layout (two-filters-per
 PACKED_HIST = 64  # the covariance history slabs are in that layout (same kernel only)
 
 PACKED_REFUSED = ("packed covariances exist only where the two-filters-per-warp kernel serves the filter (even EDIM <= 32, "
-                  "no feature-track kind, REDNOSE_B200_WARP_KERNEL != single)")
+                  "no feature-track kind)")
 
 
 def packed_P_doubles(folder, name):

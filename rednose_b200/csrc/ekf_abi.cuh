@@ -83,29 +83,22 @@ struct HostCtx {
 
 constexpr int THREAD_MAX_EDIM = 6;
 
-// true when a step of filter M serves its covariance with the pair kernel (ekf_warp2.cuh), the only kernel that reads
-// and writes the packed layout; reads REDNOSE_B200_WARP_KERNEL at call time, like launch_step.  A filter with a
-// feature-track kind is never served whole by the pair kernel (its feature kinds run on the CTA kernel, which reads the
-// full layout), so its P stays full
+// true when the steps of filter M serve its covariance with the pair kernel (ekf_warp2.cuh), the only kernel that reads
+// and writes the packed layout.  A filter with a feature-track kind is never served whole by the pair kernel (its feature
+// kinds run on the CTA kernel, which reads the full layout), so its P stays full
 template <class M>
 constexpr bool pair_may_serve() { return M::EDIM > THREAD_MAX_EDIM && use_pair<M>() && !M::HAS_FEATURE_KIND; }
 
-template <class M>
-inline bool pair_serves() {
-  if constexpr (pair_may_serve<M>()) return pair_enabled();
-  else return false;
-}
-
 // doubles per filter of the packed covariance layout, 0 when the pair kernel does not serve this filter
 template <class M>
-inline int packed_P_doubles() { return pair_serves<M>() ? packed_doubles(M::EDIM) : 0; }
+constexpr int packed_P_doubles() { return pair_may_serve<M>() ? packed_doubles(M::EDIM) : 0; }
 
 // FLAG_PACKED_P or FLAG_PACKED_HIST on a launch that the pair kernel would not run: rejected before any CUDA call
 template <class M, bool FEATURE_KIND>
 inline bool check_packed_flag(int flags, const char* what) {
-  if (!(flags & (FLAG_PACKED_P | FLAG_PACKED_HIST)) || (!FEATURE_KIND && pair_serves<M>())) return true;
+  if (!(flags & (FLAG_PACKED_P | FLAG_PACKED_HIST)) || (!FEATURE_KIND && pair_may_serve<M>())) return true;
   fprintf(stderr, "[rednose_b200] %s: the packed covariance layout (%s) exists only for the two-filters-per-warp kernel "
-                  "(even EDIM <= 32, no feature kinds, REDNOSE_B200_WARP_KERNEL != single)\n", what,
+                  "(even EDIM <= 32, no feature kinds)\n", what,
           (flags & FLAG_PACKED_P) ? "P" : "history slabs");
   last_status() = (int)cudaErrorNotSupported;
   return false;
@@ -134,15 +127,13 @@ inline void launch_step(const StepArgs<M::NG>& a, cudaStream_t st) {
       ekf_step_thread<M, K, PRED, UPD><<<grid, 128, 0, st>>>(a);
     }
   } else if constexpr (M::EDIM <= 32 && !K::HAS_HE) {
-    if (use_tma<M>() && (reinterpret_cast<uintptr_t>(a.P) & 15u)) {
-      fprintf(stderr, "[rednose_b200] P must be 16-byte aligned (bulk-copy staging of covariance tiles)\n");
-      last_status() = (int)cudaErrorMisalignedAddress;
-      return;
-    }
-    bool paired = false;
-    if constexpr (use_pair<M>()) paired = pair_enabled();
-    if constexpr (use_pair<M>()) if (paired) {
+    if constexpr (use_pair<M>()) {
       // two filters per warp (ekf_warp2.cuh): 128-bit accesses to every covariance array
+      if (reinterpret_cast<uintptr_t>(a.P) & 15u) {
+        fprintf(stderr, "[rednose_b200] P must be 16-byte aligned (bulk-copy staging of covariance tiles)\n");
+        last_status() = (int)cudaErrorMisalignedAddress;
+        return;
+      }
       if ((reinterpret_cast<uintptr_t>(a.hP_pred) | reinterpret_cast<uintptr_t>(a.hP_filt)) & 15u) {
         fprintf(stderr, "[rednose_b200] covariance history slabs must be 16-byte aligned\n");
         last_status() = (int)cudaErrorMisalignedAddress;
@@ -181,8 +172,7 @@ inline void launch_step(const StepArgs<M::NG>& a, cudaStream_t st) {
         if (phist) run(phist_kernel(std::false_type{}));
         else run(packed ? ekf_step_pair<M, K, PRED, UPD, G, false, true> : ekf_step_pair<M, K, PRED, UPD, G, false, false>);
       }
-    }
-    if (!paired) {
+    } else {
       constexpr int G = WARP_GROUP, W = WARP_CTA_WARPS;
       constexpr size_t smem = warp_smem_bytes<M, K, G, W>();
       const long long per_cta = (long long)G * W;

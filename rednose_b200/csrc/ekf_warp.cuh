@@ -1,8 +1,7 @@
-// rednose_b200 -- warp-per-filter fused predict+update kernel (6 < EDIM <= 32,
-// e.g. live_kf: DIM 23 / EDIM 22, examples/live_kf.py:97-124).
+// rednose_b200 -- warp-per-filter fused predict+update kernel (odd EDIM 7..31).
 //
-// Since the end of round 1 even-EDIM filters run ekf_step_pair (ekf_warp2.cuh: two filters per warp, same phases and
-// arithmetic, built on the primitives of this file); this kernel serves odd EDIM and REDNOSE_B200_WARP_KERNEL=single.
+// Even-EDIM filters (e.g. live_kf: DIM 23 / EDIM 22, examples/live_kf.py:97-124) run ekf_step_pair (ekf_warp2.cuh: two
+// filters per warp, same phases and arithmetic, built on the primitives of this file); this kernel serves odd EDIM.
 //
 // A warp owns a GROUP of G consecutive filters and walks through three phases:
 //
@@ -35,12 +34,10 @@ namespace rnb {
 
 constexpr int WARP_GROUP = 14;   // filters per warp group (leaf phase uses WARP_GROUP of the 32 lanes)
 constexpr int WARP_CTA_WARPS = 1;   // warps per CTA (warps never synchronise with each other)
-// covariance tile ring per warp = bulk loads in flight per warp; deeper rings cost occupancy and were slower
-constexpr int WARP_STAGES = 1;
 
 constexpr int even_up(int n) { return (n + 1) & ~1; }
 
-// ---- TMA (cp.async.bulk) + mbarrier primitives; SASS: UBLKCP / SYNCS ----
+// ---- TMA (cp.async.bulk) + mbarrier primitives (ekf_step_pair's tile ring and staging); SASS: UBLKCP / SYNCS ----
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
 __device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) {
   asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count) : "memory");
@@ -97,15 +94,9 @@ __device__ __forceinline__ void vec_load(const double* src, double (&v)[N]) {
   for (int i = 0; i < N; i += 2) { const double2 t = *reinterpret_cast<const double2*>(src + i); v[i] = t.x; v[i + 1] = t.y; }
 }
 
-template <class M>
-constexpr bool use_tma() { return (M::EDIM * M::EDIM) % 2 == 0; }  // bulk copies move multiples of 16 bytes
-
 template <class M, class K, int G>
 struct WarpScratch {
   using L = RowLayout<M, K>;
-  static constexpr int NST = use_tma<M>() ? WARP_STAGES : 0;
-  alignas(128) double tile[(NST > 0 ? NST : 1) * (use_tma<M>() ? M::EDIM * M::EDIM : 2)];  // covariance tiles (TMA ring)
-  alignas(8) uint64_t full[NST > 0 ? NST : 1];                                              // "tile landed" mbarriers
   alignas(16) double rows[G * L::STRIDE];
   // exchange row stride = 2 (mod 4) doubles: rows start 16-byte aligned and the lanes that read a whole row each
   // (128-bit accesses, one row per lane) hit distinct bank groups; the column writes (lane l -> element l) are
@@ -186,7 +177,7 @@ __global__ void __launch_bounds__(W * 32, WARP_MIN_WARPS / W) ekf_step_warp(cons
   using L = RowLayout<M, K>;
   constexpr int RS = L::STRIDE;
   constexpr int EXS = WarpScratch<M, K, G>::EXS;
-  static_assert(E <= 32, "warp-per-filter kernel needs EDIM <= 32");
+  static_assert(E <= 32 && E % 2 == 1, "warp-per-filter kernel: odd EDIM <= 32 (even EDIM runs ekf_step_pair)");
   static_assert(G <= 32, "group size");
   extern __shared__ __align__(128) unsigned char smem_raw[];
   WarpScratch<M, K, G>& s = reinterpret_cast<WarpScratch<M, K, G>*>(smem_raw)[threadIdx.x >> 5];
@@ -217,25 +208,6 @@ __global__ void __launch_bounds__(W * 32, WARP_MIN_WARPS / W) ekf_step_warp(cons
   };
   auto hid_of = [&](int f) -> long long { return __shfl_sync(0xffffffffu, myhid, f); };   // gather lists only
 
-  constexpr bool TMA = use_tma<M>();
-  constexpr int NST = TMA ? WARP_STAGES : 1;
-  constexpr uint32_t TILE_BYTES = E * E * sizeof(double);
-  uint32_t it = 0;  // tiles consumed so far by this warp (ring position / mbarrier parity)
-  if constexpr (TMA) {
-    if (lane == 0) {
-#pragma unroll
-      for (int st = 0; st < NST; ++st) mbar_init(&s.full[st], 1);
-      asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-      fence_async_smem();
-    }
-    __syncwarp();
-  }
-  // producer side of the tile ring: one elected lane arms the barrier and issues the bulk copy
-  auto issue_load = [&](long long fid, uint32_t slot) {
-    mbar_expect_tx(&s.full[slot], TILE_BYTES);
-    tma_load_1d(s.tile + slot * (E * E), a.P + fid * (long long)(E * E), TILE_BYTES, &s.full[slot]);
-  };
-
   // diagonal process noise: this lane's entry, fetched once per warp
   double qdiag = 0.0;
   if (PRED && (a.flags & FLAG_Q_DIAG)) qdiag = __ldg(a.Q + col * E + col);
@@ -243,19 +215,6 @@ __global__ void __launch_bounds__(W * 32, WARP_MIN_WARPS / W) ekf_step_warp(cons
   const int n_obs = UPD ? a.n_obs : 1;
   for (int o = 0; o < n_obs; ++o) {
     const bool do_pred = PRED && o == 0;
-    if constexpr (TMA) {
-      if (o > 0) {
-        // this warp's own plain stores of P (previous observation pass) must be visible to the bulk-copy engine
-        asm volatile("fence.proxy.async;" ::: "memory");
-        __syncwarp();
-      }
-      // prefetch the first covariance tiles of the group; they land while the leaf phase runs
-#pragma unroll
-      for (int k = 0; k < NST; ++k) {
-        const long long fid = fid_of(k < ng ? k : 0);
-        if (lane == 0 && k < ng) issue_load(fid, (it + k) % NST);
-      }
-    }
 
     // ---- stage this group's small per-filter records into the rows (coalesced) ----
     // every global load of the block (x, z, R, dt) is issued before the first shared-memory store that depends on
@@ -354,36 +313,11 @@ __global__ void __launch_bounds__(W * 32, WARP_MIN_WARPS / W) ekf_step_warp(cons
       if constexpr (GATHER) { hb = hid_of(f); rec = hb >= 0; }
       double* row = s.rows + f * RS;
       double p[E];
-      const uint32_t slot = it % NST;
-      double* tile = s.tile + (TMA ? slot * (E * E) : 0);
-      // the F value slots are loaded after the tile wait: loaded before it they held 74 more registers live and
-      // spilled inside the per-filter loop
       double fv[L::NFp];
-      if constexpr (TMA) {
-        mbar_wait(&s.full[slot], (it / NST) & 1u);
-        // P is symmetric: read ROW `lane` (contiguous, 128-bit accesses) as column `lane`
-        if constexpr (E % 2 == 0) {
+      // column `lane` of P straight from global memory: an odd-EDIM tile is no multiple of the 16 bytes a bulk copy moves
+      const double* Pg = a.P + b * (long long)(E * E) + col;
 #pragma unroll
-          for (int i = 0; i < E; i += 2) {
-            const double2 t = *reinterpret_cast<const double2*>(tile + col * E + i);
-            p[i] = t.x; p[i + 1] = t.y;
-          }
-        } else {
-#pragma unroll
-          for (int i = 0; i < E; ++i) p[i] = tile[i * E + col];
-        }
-        // the slot is free as soon as every lane has its column in registers: refill it at once,
-        // keeping NST bulk loads in flight per warp
-        const long long nfid = fid_of(f + NST < ng ? f + NST : 0);
-        fence_async_smem();   // generic-proxy reads of the tile ordered before the async-proxy refill (see ekf_warp2.cuh)
-        __syncwarp();   // every lane has read its column before the slot is overwritten
-        if (lane == 0 && f + NST < ng) issue_load(nfid, slot);
-      } else {
-        const double* Pg = a.P + b * (long long)(E * E) + col;
-#pragma unroll
-        for (int i = 0; i < E; ++i) p[i] = Pg[i * E];
-      }
-      ++it;
+      for (int i = 0; i < E; ++i) p[i] = Pg[i * E];
 
       if (do_pred) {
         vec_load(row + L::OFF_FV, fv);
@@ -509,7 +443,6 @@ __global__ void __launch_bounds__(W * 32, WARP_MIN_WARPS / W) ekf_step_warp(cons
         }
       }
 
-      // plain coalesced stores from registers: a bulk store of the tile was measured and was not faster
       if (act) {
         double* Pg = a.P + b * (long long)(E * E) + col;
 #pragma unroll

@@ -18,7 +18,6 @@
 #pragma once
 #include "ekf_warp.cuh"
 #include "ekf_packed.cuh"
-#include <cstdlib>
 
 namespace rnb {
 
@@ -27,9 +26,9 @@ constexpr int PAIR_MIN_WARPS = 8;   // ~200 live values per lane: 255 registers,
 
 // Depth of the covariance tile ring (pairs in flight per warp).  A packed pair (live_kf: 4 224 B) is little more than half
 // a full one (7 744 B), so with the packed layout two slots cost about what one full slot does and the warp keeps two
-// pairs in flight at 8 warps per SM; the full layout (unflagged ABI, host_step) keeps WARP_STAGES slots of its size.
+// pairs in flight at 8 warps per SM; the full layout (unflagged ABI, host_step) keeps one slot of its size.
 template <bool PACKED>
-constexpr int pair_stages() { return PACKED ? 2 : WARP_STAGES; }
+constexpr int pair_stages() { return PACKED ? 2 : 1; }
 
 template <class M, class K, int G, bool PACKED>
 struct PairScratch {
@@ -540,13 +539,5 @@ constexpr size_t pair_smem_bytes() { return sizeof(PairScratch<M, K, G, PACKED>)
 
 template <class M>
 constexpr bool use_pair() { return M::EDIM % 2 == 0 && M::EDIM <= 32; }
-
-// run-time escape hatch (and the way the tests reach ekf_step_warp on an even-EDIM filter):
-// REDNOSE_B200_WARP_KERNEL=single selects the one-filter-per-warp kernel; read at every launch (a getenv is
-// nothing next to a kernel launch) so that a test can flip it inside one process
-inline bool pair_enabled() {
-  const char* e = getenv("REDNOSE_B200_WARP_KERNEL");
-  return !(e && e[0] == 's');
-}
 
 }  // namespace rnb

@@ -231,7 +231,7 @@ def _shape(edim, **spec):
   return type(f'Shape{edim}', (ShapeFilter,), dict(name=f'shape_e{edim}', edim=edim, spec=spec, __module__=__name__))
 
 
-# one filter per dispatch boundary: thread (1, 4, 6), single warp without TMA (odd 7, 31), pair (8, 16, 24, 28, 32)
+# one filter per dispatch boundary: thread (1, 4, 6), one filter per warp (odd 7, 31), pair (8, 16, 24, 28, 32)
 SHAPES = [
   _shape(1, zdims=(1,), maha_kinds=(1,)),
   _shape(4, zdims=(1, 3, 4), maha_kinds=(3,), ea_kind=2, n_globals=1),

@@ -45,21 +45,18 @@ def _step(ffi, lib, name, kind, flags, B=0):
 
 
 @pytest.mark.parametrize("cls", MSCKF_SHAPES, ids=IDS)
-def test_full_covariance_layout_under_the_engines_flags(cls, monkeypatch):
+def test_full_covariance_layout_under_the_engines_flags(cls):
   """A filter with a feature-track kind keeps P full: the CTA kernel, which runs its feature kinds, reads only that
   layout.  Every kind is accepted with the flags BatchedEKF passes (B = 0: an accepted launch returns before any CUDA
   call), and the packed flag stays refused for feature kinds."""
   ffi, lib = _load(cls)
-  for env in (None, "single"):
-    if env:
-      monkeypatch.setenv("REDNOSE_B200_WARP_KERNEL", env)
-    packed = getattr(lib, f"{cls.name}_packed_P_doubles")()
-    assert packed == 0, (env, packed)
-    pflag = PACKED_P if packed else 0                 # what BatchedEKF._P_arg adds to every launch
-    for kind in cls.kinds():
-      assert _step(ffi, lib, cls.name, kind, 3 | pflag) == 0, kind
-    for kind in cls.feature_kinds():
-      assert _step(ffi, lib, cls.name, kind, 3 | PACKED_P) == CUDA_NOT_SUPPORTED
+  packed = getattr(lib, f"{cls.name}_packed_P_doubles")()
+  assert packed == 0, packed
+  pflag = PACKED_P if packed else 0                   # what BatchedEKF._P_arg adds to every launch
+  for kind in cls.kinds():
+    assert _step(ffi, lib, cls.name, kind, 3 | pflag) == 0, kind
+  for kind in cls.feature_kinds():
+    assert _step(ffi, lib, cls.name, kind, 3 | PACKED_P) == CUDA_NOT_SUPPORTED
 
 
 @pytest.mark.parametrize("cls", MSCKF_SHAPES, ids=IDS)

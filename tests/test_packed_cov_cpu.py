@@ -128,7 +128,7 @@ def _gen(cls):
   return load_code(d, cls.name)
 
 
-def test_packed_doubles_per_filter(gen_dir, monkeypatch):
+def test_packed_doubles_per_filter(gen_dir):
   from rednose_b200.filters.kinematic import KinematicKalman
   from rednose_b200.filters.live import LiveKalman
   from rednose_b200.filters.msckf import MsckfKalman
@@ -138,8 +138,6 @@ def test_packed_doubles_per_filter(gen_dir, monkeypatch):
   assert live.live_packed_P_doubles() == 264
   assert kin.kinematic_packed_P_doubles() == 0       # EDIM 2: thread-per-filter kernel
   assert msckf.msckf_packed_P_doubles() == 0         # EDIM > 32: CTA kernel
-  monkeypatch.setenv("REDNOSE_B200_WARP_KERNEL", "single")   # read at call time
-  assert live.live_packed_P_doubles() == 0
 
 
 def _step(ffi, lib, name, kind, E, flags, B=0):
@@ -149,11 +147,12 @@ def _step(ffi, lib, name, kind, E, flags, B=0):
   return getattr(lib, f"{name}_cuda_status")()
 
 
-def test_flag_rejected_where_the_pair_kernel_does_not_run(gen_dir, monkeypatch):
+def test_flag_rejected_where_the_pair_kernel_does_not_run(gen_dir):
   """B = 0: an accepted launch returns before any CUDA call, so acceptance is checkable without a GPU too."""
   from rednose_b200.filters.kinematic import KinematicKalman
   from rednose_b200.filters.live import LiveKalman
   from rednose_b200.filters.msckf import MsckfKalman
+  from tests.shapes import BY_NAME
   ffi, live = _gen(LiveKalman)
   assert _step(ffi, live, "live", 12, 22, 3 | PACKED_P) == 0
   ffi_k, kin = _gen(KinematicKalman)
@@ -167,12 +166,14 @@ def test_flag_rejected_where_the_pair_kernel_does_not_run(gen_dir, monkeypatch):
   # host buffers are always full
   live.live_host_step_12(x, P, P, ffi.NULL, 0.01, z, R, ffi.NULL, 1, 1, qi, 1, PACKED_P)
   assert live.live_cuda_status() == CUDA_NOT_SUPPORTED
-  monkeypatch.setenv("REDNOSE_B200_WARP_KERNEL", "single")
-  assert _step(ffi, live, "live", 12, 22, 3 | PACKED_P) == CUDA_NOT_SUPPORTED
-  live.live_batch_predict(x, P, P, ffi.NULL, 0.01, 0, qi, 1, PACKED_P, ffi.NULL, ffi.NULL, ffi.NULL)
-  assert live.live_cuda_status() == CUDA_NOT_SUPPORTED
-  live.live_batch_update_12(x, P, z, R, ffi.NULL, 1, 0, qi, 1, PACKED_P, ffi.NULL, ffi.NULL, ffi.NULL)
-  assert live.live_cuda_status() == CUDA_NOT_SUPPORTED
-  live.live_batch_maha_12(x, P, z, R, ffi.NULL, 0, PACKED_P, out, ffi.NULL)
-  assert live.live_cuda_status() == CUDA_NOT_SUPPORTED
-  assert live.live_cuda_status() == 0
+  ffi_7, e7 = _gen(BY_NAME["shape_e7"])               # odd EDIM: one filter per warp
+  assert _step(ffi_7, e7, "shape_e7", 1, 7, PACKED_P) == CUDA_NOT_SUPPORTED
+  x, P, z, R, out = (ffi_7.new("double[]", n) for n in (7, 49, 1, 1, 1))
+  qi = ffi_7.new("int[]", [0])
+  e7.shape_e7_batch_predict(x, P, P, ffi_7.NULL, 0.01, 0, qi, 0, PACKED_P, ffi_7.NULL, ffi_7.NULL, ffi_7.NULL)
+  assert e7.shape_e7_cuda_status() == CUDA_NOT_SUPPORTED
+  e7.shape_e7_batch_update_1(x, P, z, R, ffi_7.NULL, 1, 0, qi, 0, PACKED_P, ffi_7.NULL, ffi_7.NULL, ffi_7.NULL)
+  assert e7.shape_e7_cuda_status() == CUDA_NOT_SUPPORTED
+  e7.shape_e7_batch_maha_1(x, P, z, R, ffi_7.NULL, 0, PACKED_P, out, ffi_7.NULL)
+  assert e7.shape_e7_cuda_status() == CUDA_NOT_SUPPORTED
+  assert e7.shape_e7_cuda_status() == 0

@@ -79,7 +79,7 @@ def _rts(ffi, lib, name, which, D=64, E=64):
 RTS = ("rts", "rts_segment", "rts_ragged")
 
 
-def test_packed_history_refused_where_the_pair_kernel_does_not_run(gen_dir, monkeypatch):
+def test_packed_history_refused_where_the_pair_kernel_does_not_run(gen_dir):
   """B = 0: an accepted launch returns before any CUDA call, so acceptance is checkable without a GPU too."""
   from rednose_b200.filters.kinematic import KinematicKalman
   from rednose_b200.filters.live import LiveKalman
@@ -94,7 +94,15 @@ def test_packed_history_refused_where_the_pair_kernel_does_not_run(gen_dir, monk
   assert all(_rts(ffi_k, kin, "kinematic", w) == CUDA_NOT_SUPPORTED for w in RTS)
   _, (ffi_7, e7) = _gen(BY_NAME["shape_e7"])             # odd EDIM: one filter per warp
   assert _step(ffi_7, e7, "shape_e7", 1, 7, PACKED_HIST) == CUDA_NOT_SUPPORTED
+  x7, P7, z7, R7 = (ffi_7.new("double[]", n) for n in (7, 49, 1, 1))
+  q7 = ffi_7.new("int[]", [0])
+  e7.shape_e7_batch_predict(x7, P7, P7, ffi_7.NULL, 0.01, 0, q7, 0, PACKED_HIST, ffi_7.NULL, P7, ffi_7.NULL)
+  assert e7.shape_e7_cuda_status() == CUDA_NOT_SUPPORTED
+  e7.shape_e7_batch_update_1(x7, P7, z7, R7, ffi_7.NULL, 1, 0, q7, 0, PACKED_HIST, ffi_7.NULL, P7, ffi_7.NULL)
+  assert e7.shape_e7_cuda_status() == CUDA_NOT_SUPPORTED
   assert all(_rts(ffi_7, e7, "shape_e7", w) == CUDA_NOT_SUPPORTED for w in RTS)
+  assert e7.shape_e7_cuda_status() == CUDA_NOT_SUPPORTED   # a refused call also latches its status, like _hist_idx
+  assert e7.shape_e7_cuda_status() == 0
   _, (ffi_m, msckf) = _gen(MsckfKalman)                   # EDIM > 32 and feature kinds: CTA kernel
   kinds = sorted(int(s.rsplit("_", 1)[1]) for s in dir(msckf) if s.startswith("msckf_batch_step_") and not s.endswith("_idx"))
   for k in kinds:
@@ -104,14 +112,6 @@ def test_packed_history_refused_where_the_pair_kernel_does_not_run(gen_dir, monk
   qi = ffi.new("int[]", [3])
   live.live_host_step_12(x, P, P, ffi.NULL, 0.01, z, R, ffi.NULL, 1, 1, qi, 1, PACKED_HIST)   # host buffers are always full
   assert live.live_cuda_status() == CUDA_NOT_SUPPORTED
-  monkeypatch.setenv("REDNOSE_B200_WARP_KERNEL", "single")
-  assert _step(ffi, live, "live", 12, 22, 3 | PACKED_HIST) == CUDA_NOT_SUPPORTED
-  live.live_batch_predict(x, P, P, ffi.NULL, 0.01, 0, qi, 1, PACKED_HIST, ffi.NULL, P, ffi.NULL)
-  assert live.live_cuda_status() == CUDA_NOT_SUPPORTED
-  live.live_batch_update_12(x, P, z, R, ffi.NULL, 1, 0, qi, 1, PACKED_HIST, ffi.NULL, P, ffi.NULL)
-  assert live.live_cuda_status() == CUDA_NOT_SUPPORTED
-  assert all(_rts(ffi, live, "live", w) == CUDA_NOT_SUPPORTED for w in RTS)
-  assert live.live_cuda_status() == CUDA_NOT_SUPPORTED   # a refused call also latches its status, like _hist_idx
   assert live.live_cuda_status() == 0
 
 

@@ -243,12 +243,11 @@ def test_ragged_packed_history_through_the_scheduler():
     assert ex < TIGHT and eP < TIGHT, (f, ex, eP)
 
 
-def test_packed_history_refused(monkeypatch):
+def test_packed_history_refused():
   """(g) ValueError from new_history / new_ragged_history where the filter has no packed layout: kinematic (thread
-  kernel), shape_e7 (odd EDIM), an MSCKF with a feature kind (CTA kernel), and live under REDNOSE_B200_WARP_KERNEL=single."""
+  kernel), shape_e7 (odd EDIM) and an MSCKF with a feature kind (CTA kernel)."""
   from rednose_b200.filters import ensure_generated
   from rednose_b200.filters.kinematic import KinematicKalman
-  from rednose_b200.filters.live import LiveKalman
   from tests.msckf_shapes import BY_NAME as MSCKF_BY_NAME, batch as msckf_batch
   from tests.util import kinematic_batch
   xk, Pk, Qk, _, _ = kinematic_batch(4, seed=1)
@@ -266,8 +265,3 @@ def test_packed_history_refused(monkeypatch):
       e.new_history(3, packed=True)
     with pytest.raises(ValueError, match="two-filters-per-warp"):
       e.new_ragged_history(3, packed=True)
-  monkeypatch.setenv("REDNOSE_B200_WARP_KERNEL", "single")
-  x, P, Q = live_batch(4, seed=1)
-  e = _engine(ensure_generated(LiveKalman), "live", x, P, Q, [3], {})
-  with pytest.raises(ValueError, match="two-filters-per-warp"):
-    e.new_history(3, packed=True)

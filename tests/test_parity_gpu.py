@@ -500,40 +500,6 @@ def test_rts_scalar_fallback_on_the_kinematic_model(gen_dir, oracle_dir):
     assert state_err(xs[:, b], xr) < 1e-9 and cov_err(Ps[:, b], Pr) < 1e-9
 
 
-@pytest.fixture
-def single_warp_kernel(monkeypatch):
-  """Select ekf_step_warp (one filter per warp, the kernel odd-EDIM filters use) instead of ekf_step_pair."""
-  monkeypatch.setenv("REDNOSE_B200_WARP_KERNEL", "single")
-
-
-@pytest.mark.parametrize("kind", [3, 4, 10, 13])
-def test_single_filter_per_warp_kernel_fused_step(gen_dir, oracle_dir, single_warp_kernel, kind):
-  test_live_fused_step_every_kind(gen_dir, oracle_dir, kind)
-
-
-def test_single_filter_per_warp_kernel_other_paths(gen_dir, oracle_dir, single_warp_kernel):
-  test_live_predict_and_update_separately(gen_dir, oracle_dir)
-  test_multiple_observations_per_predict(gen_dir, oracle_dir)
-  test_ragged_scheduler_matches_per_filter_driving(gen_dir, oracle_dir)
-  test_edge_batches_empty_single_and_ragged_tail(gen_dir, oracle_dir)
-  test_history_slabs_equal_separate_predict_update(gen_dir, oracle_dir)
-
-
-def test_pair_and_single_kernels_agree_to_rounding(gen_dir, oracle_dir, monkeypatch):
-  """Same arithmetic, same order per column: the two lane mappings give bitwise-equal x and P."""
-  o = Oracle(oracle_dir, "live")
-  B = 777   # odd: the last pair of the last group has an idle half
-  x, P, Qm = live_batch(B, seed=5)
-  z, R = live_obs(o, 10, x)
-  out = []
-  for mode in ("pair", "single"):
-    monkeypatch.setenv("REDNOSE_B200_WARP_KERNEL", mode)
-    e = _engine(gen_dir, "live", x, P, Qm, quaternion_idxs=[3])
-    y = e.step(10, 0.01, z, R)
-    out.append((e.state().copy(), e.covs().copy(), y.cpu().numpy().copy()))
-  assert state_err(out[0][0], out[1][0]) < 1e-14 and cov_err(out[0][1], out[1][1]) < 1e-14 and state_err(out[0][2], out[1][2]) < 1e-14
-
-
 def test_dense_process_noise(gen_dir, oracle_dir):
   """A Q with off-diagonal terms takes the dense dt*Q path of the kernels (the diagonal fast path is what every
   other live test runs, examples/live_kf.py's Q being diagonal); ekf_c.c:27-28."""

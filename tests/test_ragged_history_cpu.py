@@ -57,10 +57,9 @@ def _lib(cls):
   return load_code(ensure_generated(cls), cls.name)
 
 
-def test_recording_step_rejects_bad_arguments_before_any_cuda_call(monkeypatch):
+def test_recording_step_rejects_bad_arguments_before_any_cuda_call():
   """Every case returns its status without touching the device (so it runs here without one)."""
   from rednose_b200.filters.live import LiveKalman
-  monkeypatch.delenv("REDNOSE_B200_WARP_KERNEL", raising=False)
   ffi, lib = _lib(LiveKalman)
   assert lib.live_cuda_status() == 0
   x, P, Q, z, R = (ffi.new("double[]", n) for n in (24, 22 * 22, 22 * 22, 4, 10))

@@ -34,7 +34,7 @@ def _dev(a):
 def _lockstep_case(name):
   """(folder, engine name, x, P, Q, quats, [(kind, z, R, ea)] per tick) of one kernel path."""
   from rednose_b200.filters import ensure_generated
-  if name in ("live", "live_single"):
+  if name == "live":
     from rednose_b200.filters.live import LiveKalman
     x, P, Q = live_batch(45, seed=3)
     ticks = []
@@ -66,13 +66,11 @@ def _lockstep_case(name):
   return ensure_generated(cls), cls.name, x, P, Q, cls.quat_idxs(), ticks
 
 
-@pytest.mark.parametrize("case", ["live", "kinematic", "shape_e7", "live_single", "msckf_e18", "msckf_e28"])
-def test_lockstep_stream_equals_lockstep_recording_bit_for_bit(case, monkeypatch):
+@pytest.mark.parametrize("case", ["live", "kinematic", "shape_e7", "msckf_e18", "msckf_e28"])
+def test_lockstep_stream_equals_lockstep_recording_bit_for_bit(case):
   """Every filter observes every tick with the same kind and time: RaggedScheduler(history=) + rts_smooth(ragged) ==
   step_recorded + rts_smooth(History), torch.equal on x, P, the four slabs and the smoothed rows."""
   from rednose_b200.scheduler import RaggedScheduler
-  if case == "live_single":
-    monkeypatch.setenv("REDNOSE_B200_WARP_KERNEL", "single")
   folder, name, x, P, Q, q, ticks = _lockstep_case(case)
   B, T = x.shape[0], len(ticks)
   a, b = _engine(folder, name, x, P, Q, q), _engine(folder, name, x, P, Q, q)

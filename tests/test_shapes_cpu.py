@@ -37,13 +37,11 @@ def test_main_block_above_32_is_refused_before_nvcc(tmp_path):
 
 
 @pytest.mark.parametrize("cls", SHAPES, ids=IDS)
-def test_dispatch_facts(cls, monkeypatch):
+def test_dispatch_facts(cls):
   _, lib = _load(cls)
   E = cls.edim
   want = 4 * (E // 2) * (E // 2 + 1) // 2 if cls.step_kernel() == "pair" else 0
   assert getattr(lib, f"{cls.name}_packed_P_doubles")() == want
-  monkeypatch.setenv("REDNOSE_B200_WARP_KERNEL", "single")
-  assert getattr(lib, f"{cls.name}_packed_P_doubles")() == 0
 
 
 def _fd(fun, x0, h=1e-6):
