@@ -17,6 +17,8 @@ shrinks a live history step from 8 112 to 4 592 bytes; ``unpack_P`` turns any pa
 """
 from __future__ import annotations
 
+import math
+
 import numpy as np
 import torch
 
@@ -29,9 +31,18 @@ SHARED_R = 8
 AUGMENT = 16   # fused clone-window shift (CTA kernel only)
 PACKED_P = 32  # P is in the packed lower-block-triangle layout (two-filters-per-warp kernel only)
 PACKED_HIST = 64  # the covariance history slabs are in that layout (same kernel only)
+MAIN_HIST = 128   # the predicted-covariance history slab keeps the main block only (EDIM > 32; set by the _mainhist entry points)
 
 PACKED_REFUSED = ("packed covariances exist only where the two-filters-per-warp kernel serves the filter (even EDIM <= 32, "
                   "no feature-track kind)")
+MAIN_PRED_REFUSED = "main-block prediction histories exist only above EDIM 32 (an MSCKF smoothed on its main block)"
+
+
+def main_pred_doubles(folder, name):
+  """Doubles per filter-step of the main-block prediction history of filter `name` (MEDIM^2), 0 where it does not exist
+  (EDIM <= 32)."""
+  _, lib = load_code(folder, name)
+  return int(getattr(lib, f"{name}_main_pred_doubles")())
 
 
 def packed_P_doubles(folder, name):
@@ -70,6 +81,8 @@ class BatchedEKF:
     # covariance storage: the full buffer `_Pf` and, when the pair kernel serves this filter, the packed resident buffer
     # `_Pk`; `_full_owns` says which of the two holds the current P
     self._packed_doubles = int(getattr(self._lib, f"{name}_packed_P_doubles")())
+    # MEDIM^2 above EDIM 32 (a main-block prediction history is available), 0 elsewhere
+    self._main_pred_doubles = int(getattr(self._lib, f"{name}_main_pred_doubles")())
     self._Pf = P0.contiguous().clone()
     self._full_owns = True
     self._Pk = None
@@ -298,10 +311,13 @@ class BatchedEKF:
     self._check(f"batch_step_{kind}_idx")
     return z
 
-  def step(self, kind, dt, z, R, ea=None, hist_pred=None, hist_filt=None, augment=False):
+  def step(self, kind, dt, z, R, ea=None, hist_pred=None, hist_filt=None, augment=False, hist_pred_last=None):
     """Fused predict(dt) + update(kind): one kernel launch, P read and written once.  augment=True also shifts the MSCKF
     clone window (predict_and_update_batch(..., augment=True), ekf_sym.py:527-528): inside the same launch for filters on
-    the CTA-per-filter kernel (EDIM > 32), as a second launch otherwise."""
+    the CTA-per-filter kernel (EDIM > 32), as a second launch otherwise.
+
+    hist_pred_last [B, EDIM, EDIM] (EDIM > 32): record a main-block prediction history -- hist_pred's covariance row is
+    then [B, MEDIM, MEDIM] and receives the main block of P_{k+1|k}, hist_pred_last the whole of it."""
     keep, dt_ptr, dt_s = self._dt_args(dt)
     z, R, ea, n_obs, flags = self._obs_args(z, R, ea)
     fused_aug = bool(augment) and self.dim_err > 32
@@ -309,13 +325,21 @@ class BatchedEKF:
       flags |= AUGMENT
     hxp, hPp = (hist_pred if hist_pred is not None else (None, None))
     hxf, hPf = (hist_filt if hist_filt is not None else (None, None))
-    hflag = self._hist_flag(hPp, hPf)
+    if hist_pred_last is None:
+      hflag = self._hist_flag(hPp, hPf)
+      fn, last = f"{self.name}_batch_step_{kind}", ()
+    else:
+      me = self._main_block_dim()
+      assert hPp is None or tuple(hPp.shape[-2:]) == (me, me), (tuple(hPp.shape), me)
+      assert tuple(hist_pred_last.shape) == (self.B, self.dim_err, self.dim_err), tuple(hist_pred_last.shape)
+      hflag = self._hist_flag(hPf)
+      fn, last = f"{self.name}_batch_mainhist_step_{kind}", (self._p(hist_pred_last),)
     P, pflag = self._P_arg()
     with torch.cuda.device(self.device):
-      getattr(self._lib, f"{self.name}_batch_step_{kind}")(
+      getattr(self._lib, fn)(
         self._p(self.x), P, self._cp(self.Q), dt_ptr, dt_s, self._p(z), self._cp(R), self._cp(ea),
         n_obs, self.B, self._quat, self._nquat, flags | pflag | hflag, self._p(hxp), self._p(hPp), self._p(hxf), self._p(hPf),
-        self._stream())
+        *last, self._stream())
     self.launches += 1
     self._check(f"batch_step_{kind}")
     if augment and not fused_aug:
@@ -415,12 +439,25 @@ class BatchedEKF:
       raise ValueError(f"filter '{self.name}': packed histories are not available: {PACKED_REFUSED}")
     return self._packed_doubles
 
-  def new_history(self, T, packed=False):
+  def _main_block_dim(self):
+    return math.isqrt(self._main_pred_doubles)
+
+  def new_history(self, T, packed=False, main_pred=False):
     """Device slabs for a T-step history, time-major: what the reference keeps as the list of
     9-tuples returned by predict_and_update_batch (ekf_sym.py:531): x_{k|k-1}, x_{k|k}, P_{k|k-1}, P_{k|k}, t.
 
     packed=True records the covariances in the packed layout of the resident P ([T, B, packed doubles]: 57 % of the
-    bytes of a live history step); raises ValueError where this filter has no packed layout."""
+    bytes of a live history step); raises ValueError where this filter has no packed layout.
+
+    main_pred=True (EDIM > 32, an MSCKF) keeps only the main block of each predicted covariance, P_pred [T, B, MEDIM,
+    MEDIM], plus the full prediction of the newest step, P_pred_last [B, EDIM, EDIM]: all the smoother reads of them
+    (59 152 instead of 109 072 bytes per msckf step).  Raises ValueError at EDIM <= 32 and together with packed=True."""
+    if main_pred:
+      if packed:
+        raise ValueError("a main-block prediction history is in the full covariance layout: packed=True does not apply")
+      if not self._main_pred_doubles:
+        raise ValueError(f"filter '{self.name}': EDIM {self.dim_err}: {MAIN_PRED_REFUSED}")
+      return History(T, self.B, self.dim_x, self.dim_err, self.device, main_block=self._main_block_dim())
     return History(T, self.B, self.dim_x, self.dim_err, self.device, self._history_doubles(packed))
 
   def new_ragged_history(self, T, packed=False):
@@ -438,7 +475,7 @@ class BatchedEKF:
       self.filter_time = t
     dt = t - self.filter_time
     y = self.step(kind, dt, z, R, ea, hist_pred=(hist.x_pred[k], hist.P_pred[k]), hist_filt=(hist.x_filt[k], hist.P_filt[k]),
-                  augment=augment)
+                  augment=augment, hist_pred_last=hist.P_pred_last)
     self.filter_time = t
     hist.t_host[k] = float(t)
     hist.n += 1
@@ -450,7 +487,8 @@ class BatchedEKF:
     Returns (xs [T, B, DIM], Ps [T, B, EDIM, EDIM]) on the device.  `norm_quats` normalises the quaternion(s)
     at `quaternion_idxs` the way the reference normalises its hard-coded slice 3:7.  A packed history (new_history(T,
     packed=True)) gives packed Ps [T, B, packed doubles] (see unpack_P), and `out` / `terminal` covariances are packed
-    like it.
+    like it.  A main-block prediction history (new_history(T, main_pred=True)) gives full Ps, bit for bit those of the
+    full history, and takes full `out` / `terminal` covariances.
 
     `terminal=(x [B, DIM], P [B, EDIM, EDIM])` smooths one SEGMENT of a longer history (steps k0 .. k0 + T - 2): the
     recursion starts from that smoothed estimate of step k0 + T - 1, whose history entry (the last one recorded) only
@@ -473,12 +511,14 @@ class BatchedEKF:
       xs = hist.x_filt if in_place else torch.empty_like(hist.x_filt)
       Ps = hist.P_filt if in_place else torch.empty_like(hist.P_filt)
     qi = self._ffi.new("int[]", list(quaternion_idxs) or [0])
-    sfx = "_packed" if hist.packed else ""
+    sfx = "_packed" if hist.packed else ("_mainhist" if hist.main_pred else "")
+    last = (self._cp(hist.P_pred_last),) if hist.main_pred else ()
     with torch.cuda.device(self.device):
       if terminal is None and not k0:
         getattr(self._lib, f"{self.name}_batch_rts{sfx}")(
           self._cp(hist.x_pred), self._cp(hist.P_pred), self._cp(hist.x_filt), self._cp(hist.P_filt), self._cp(hist.t), 0,
-          self._p(xs), self._p(Ps), T, self.B, qi, len(quaternion_idxs) if norm_quats else 0, 1 if norm_quats else 0, self._stream())
+          self._p(xs), self._p(Ps), T, self.B, qi, len(quaternion_idxs) if norm_quats else 0, 1 if norm_quats else 0, *last,
+          self._stream())
       else:
         xt, Pt = terminal if terminal is not None else (None, None)   # the LAST segment of a history has k0 > 0 but no terminal
         assert xt is None or (xt.is_contiguous() and Pt.is_contiguous() and xt.shape == (self.B, self.dim_x) and Pt.shape == hist.P_filt.shape[1:]), \
@@ -486,7 +526,7 @@ class BatchedEKF:
         getattr(self._lib, f"{self.name}_batch_rts_segment{sfx}")(
           self._cp(hist.x_pred), self._cp(hist.P_pred), self._cp(hist.x_filt), self._cp(hist.P_filt), self._cp(hist.t), 0,
           self._p(xs), self._p(Ps), T, self.B, qi, len(quaternion_idxs) if norm_quats else 0, 1 if norm_quats else 0,
-          self._cp(xt), self._cp(Pt), int(k0), self._stream())
+          self._cp(xt), self._cp(Pt), int(k0), *last, self._stream())
     self.launches += 1
     self._check("batch_rts")
     return xs[:T], Ps[:T]
@@ -540,15 +580,20 @@ def _cov_shape(dim_err, packed_doubles):
 
 class History:
   """Time-major device buffers of a forward pass, consumed by the RTS kernel.  `packed`: the covariance slabs are
-  [T, B, packed_doubles] in the packed layout (BatchedEKF.new_history(T, packed=True)) instead of [T, B, EDIM, EDIM]."""
+  [T, B, packed_doubles] in the packed layout (BatchedEKF.new_history(T, packed=True)) instead of [T, B, EDIM, EDIM].
+  `main_pred` (main_block = MEDIM > 0): P_pred is [T, B, MEDIM, MEDIM] and P_pred_last [B, EDIM, EDIM] holds the full
+  prediction of the newest recorded step (BatchedEKF.new_history(T, main_pred=True)); P_pred_last is None otherwise."""
 
-  def __init__(self, T, B, dim_x, dim_err, device, packed_doubles=0):
+  def __init__(self, T, B, dim_x, dim_err, device, packed_doubles=0, main_block=0):
+    assert not (packed_doubles and main_block)
     kw = dict(dtype=torch.float64, device=device)
     self.T, self.B, self.n = T, B, 0
     self.packed = bool(packed_doubles)
+    self.main_pred = bool(main_block)
     self.x_pred = torch.empty(T, B, dim_x, **kw)
     self.x_filt = torch.empty(T, B, dim_x, **kw)
-    self.P_pred = torch.empty(T, B, *_cov_shape(dim_err, packed_doubles), **kw)
+    self.P_pred = torch.empty(T, B, *((main_block, main_block) if main_block else _cov_shape(dim_err, packed_doubles)), **kw)
+    self.P_pred_last = torch.empty(B, dim_err, dim_err, **kw) if main_block else None
     self.P_filt = torch.empty(T, B, *_cov_shape(dim_err, packed_doubles), **kw)
     self.t = torch.zeros(T, **kw)
     self.t_host = np.zeros(T)          # step times are collected on the host and uploaded once, before the backward pass
@@ -558,7 +603,7 @@ class History:
     self.t.copy_(torch.as_tensor(self.t_host))
 
   def bytes(self):
-    return sum(t.numel() * 8 for t in (self.x_pred, self.x_filt, self.P_pred, self.P_filt, self.t))
+    return sum(t.numel() * 8 for t in (self.x_pred, self.x_filt, self.P_pred, self.P_pred_last, self.P_filt, self.t) if t is not None)
 
 
 class RaggedHistory:

@@ -343,6 +343,12 @@ def gen_code(folder, name, f_sym, dt_sym, x_sym, obs_eqs, dim_x, dim_err, eskf_p
     bh = bi.replace(", void *stream", ", const int *hist_row, long long hist_B, void *stream")
     hdr.append(f"int {name}_batch_step_{k}_hist_idx({bh});")
     c.append(f'extern "C" int {name}_batch_step_{k}_hist_idx({bh}) {{ return rnb::call_status([&] {{ rnb::batch_step_hist<{model}, {ks}>(ctx_(), x, P, Q, dt_arr, dt, z, R, ea, n_obs, B, quat_idxs, n_quat, flags, hx_pred, hP_pred, hx_filt, hP_filt, idx, hist_row, hist_B, stream); }}); }}\n')
+    if EDIM > 32:
+      # main-block prediction history (FLAG_MAIN_HIST): hP_pred is one row [B, MEDIM, MEDIM], hP_pred_last [B, EDIM, EDIM]
+      # the full prediction.  int result (see _hist_idx); named so that <name>_batch_step_<kind> still lists the kinds
+      bmh = bs.replace(", void *stream", ", double *hP_pred_last, void *stream")
+      hdr.append(f"int {name}_batch_mainhist_step_{k}({bmh});")
+      c.append(f'extern "C" int {name}_batch_mainhist_step_{k}({bmh}) {{ return rnb::call_status([&] {{ rnb::batch_step_mainhist<{model}, {ks}>(ctx_(), x, P, Q, dt_arr, dt, z, R, ea, n_obs, B, quat_idxs, n_quat, flags, hx_pred, hP_pred, hx_filt, hP_filt, hP_pred_last, stream); }}); }}\n')
     bm = "const double *x, const double *P, const double *z, const double *R, const double *ea, long long B, int flags, double *out, void *stream"
     hdr.append(f"void {name}_batch_maha_{k}({bm});")
     c.append(f'extern "C" void {name}_batch_maha_{k}({bm}) {{ rnb::batch_maha<{model}, {ks}>(ctx_(), x, P, z, R, ea, B, flags, out, stream); }}\n')
@@ -375,6 +381,16 @@ def gen_code(folder, name, f_sym, dt_sym, x_sym, obs_eqs, dim_x, dim_err, eskf_p
                              ("rts_ragged", brr, f"batch_rts_ragged<{model}, true>(ctx_(), hx_pred, hP_pred, hx_filt, hP_filt, t, len, xs, Ps, T, B, quat_idxs, n_quat, norm_quats, stream)")):
     hdr.append(f"int {name}_batch_{suffix}_packed({args});")
     c.append(f'extern "C" int {name}_batch_{suffix}_packed({args}) {{ return rnb::call_status([&] {{ rnb::{call}; }}); }}\n')
+  # doubles per filter and step of a main-block prediction history (MEDIM^2), 0 where it does not exist (EDIM <= 32)
+  hdr.append(f"int {name}_main_pred_doubles(void);")
+  c.append(f'extern "C" int {name}_main_pred_doubles(void) {{ return {MEDIM * MEDIM if EDIM > 32 else 0}; }}\n')
+  if EDIM > 32:
+    # the two smoothers over a main-block prediction history: hP_pred [T, B, MEDIM, MEDIM]; without a terminal estimate
+    # the recursion starts from hP_pred_last [B, EDIM, EDIM], the full prediction of the newest row
+    for suffix, args, tail in (("rts", br, ""), ("rts_segment", brs, ", x_term, P_term, k0")):
+      args = args.replace(", void *stream", ", const double *hP_pred_last, void *stream")
+      hdr.append(f"int {name}_batch_{suffix}_mainhist({args});")
+      c.append(f'extern "C" int {name}_batch_{suffix}_mainhist({args}) {{ return rnb::call_status([&] {{ rnb::batch_rts<{model}, false, true>(ctx_(), hx_pred, hP_pred, hx_filt, hP_filt, t, t_per_filter, xs, Ps, T, B, quat_idxs, n_quat, norm_quats, stream{tail if tail else ", nullptr, nullptr, 0"}, hP_pred_last); }}); }}\n')
 
   if msckf:
     ba = "double *x, double *P, long long B, void *stream"

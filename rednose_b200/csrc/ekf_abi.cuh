@@ -104,9 +104,26 @@ inline bool check_packed_flag(int flags, const char* what) {
   return false;
 }
 
+// FLAG_MAIN_HIST exists for the fused step of a filter above EDIM 32 (the CTA-per-filter kernel), without a gather list
+// and in the full covariance layout: anything else is rejected before any CUDA call
+template <class M, bool FUSED>
+inline bool check_main_hist_flag(const StepArgs<M::NG>& a, const char* what) {
+  if (!(a.flags & FLAG_MAIN_HIST)) return true;
+  const char* why = nullptr;
+  if (M::EDIM <= 32) why = "exists only above EDIM 32";
+  else if (!FUSED) why = "is recorded by the fused predict + update step only";
+  else if (a.flags & (FLAG_PACKED_P | FLAG_PACKED_HIST)) why = "cannot be combined with the packed covariance layouts";
+  else if (a.idx) why = "cannot be combined with a gather list";   // history rows (hist_row) come only with one
+  if (!why) return true;
+  fprintf(stderr, "[rednose_b200] %s: the main-block prediction history %s\n", what, why);
+  last_status() = (int)cudaErrorNotSupported;
+  return false;
+}
+
 template <class M, class K, bool PRED, bool UPD>
 inline void launch_step(const StepArgs<M::NG>& a, cudaStream_t st) {
   if (!check_packed_flag<M, K::HAS_HE>(a.flags, "ekf_step")) return;
+  if (!check_main_hist_flag<M, PRED && UPD>(a, "ekf_step")) return;
   if (a.B <= 0) return;
   if ((a.flags & FLAG_AUGMENT) && !(M::EDIM > 32 || K::HAS_HE)) {
     fprintf(stderr, "[rednose_b200] the fused augment exists only in the CTA-per-filter kernel (EDIM > 32): call <name>_batch_augment\n");
@@ -199,7 +216,11 @@ inline void launch_step(const StepArgs<M::NG>& a, cudaStream_t st) {
     }
   } else {
     if constexpr (FUSED) {
-      if (a.hist_row) launch_step_cta<M, K, PRED, UPD, true>(a, st);
+      bool main_hist = false;   // checked first: hP_pred_last shares hist_row's slot
+      if constexpr (M::EDIM > 32) main_hist = a.flags & FLAG_MAIN_HIST;
+      if (main_hist) {
+        if constexpr (M::EDIM > 32) launch_step_cta<M, K, PRED, UPD, false, true>(a, st);
+      } else if (a.hist_row) launch_step_cta<M, K, PRED, UPD, true>(a, st);
       else launch_step_cta<M, K, PRED, UPD>(a, st);
     } else {
       launch_step_cta<M, K, PRED, UPD>(a, st);
@@ -239,11 +260,13 @@ inline void batch_step(HostCtx<M>& ctx, double* x, double* P, const double* Q, c
                        double* z, const double* R, const double* ea, int n_obs, long long B,
                        const int* quat_idxs, int n_quat, int flags,
                        double* hx_pred, double* hP_pred, double* hx_filt, double* hP_filt, void* stream,
-                       const int* idx = nullptr, const int* hist_row = nullptr, long long hist_B = 0) {
+                       const int* idx = nullptr, const int* hist_row = nullptr, long long hist_B = 0,
+                       double* hP_pred_last = nullptr) {
   StepArgs<M::NG> a;
   if (!fill_common<M>(a, ctx, B, quat_idxs, n_quat, flags)) return;
   a.idx = idx;
   a.hist_row = hist_row; a.hist_B = hist_B;
+  if (hP_pred_last) a.hP_pred_last = hP_pred_last;   // shares hist_row's slot (StepArgs); the main-block step has no rows
   a.x = x; a.P = P; a.Q = Q; a.dt_arr = dt_arr; a.dt = dt;
   a.z = z; a.R = R; a.ea = (K::EADIM > 0) ? ea : nullptr; a.ea_dim = K::EADIM; a.n_obs = n_obs;
   a.hx_pred = hx_pred; a.hP_pred = hP_pred; a.hx_filt = hx_filt; a.hP_filt = hP_filt;
@@ -264,6 +287,18 @@ inline void batch_step_hist(HostCtx<M>& ctx, double* x, double* P, const double*
   }
   batch_step<M, K, true>(ctx, x, P, Q, dt_arr, dt, z, R, ea, n_obs, B, quat_idxs, n_quat, flags,
                          hx_pred, hP_pred, hx_filt, hP_filt, stream, idx, hist_row, hist_B);
+}
+
+// fused step that records one row of a main-block prediction history (FLAG_MAIN_HIST): hP_pred [B, MEDIM, MEDIM] gets
+// the main block of P_{k+1|k}, hP_pred_last [B, EDIM, EDIM] the whole of it
+template <class M, class K>
+inline void batch_step_mainhist(HostCtx<M>& ctx, double* x, double* P, const double* Q, const double* dt_arr, double dt,
+                                double* z, const double* R, const double* ea, int n_obs, long long B,
+                                const int* quat_idxs, int n_quat, int flags,
+                                double* hx_pred, double* hP_pred, double* hx_filt, double* hP_filt, double* hP_pred_last,
+                                void* stream) {
+  batch_step<M, K, true>(ctx, x, P, Q, dt_arr, dt, z, R, ea, n_obs, B, quat_idxs, n_quat, flags | FLAG_MAIN_HIST,
+                         hx_pred, hP_pred, hx_filt, hP_filt, stream, nullptr, nullptr, 0, hP_pred_last);
 }
 
 }  // namespace rnb
@@ -291,16 +326,31 @@ inline bool check_packed_hist(const char* what) {
   else return true;
 }
 
-template <class M, bool PH = false>
+// MH: a main-block prediction history (FLAG_MAIN_HIST, EDIM > 32): hP_pred is [T, B, MEDIM, MEDIM] and, without a
+// terminal estimate, the recursion starts from hP_pred_last [B, EDIM, EDIM], the full prediction of the newest row
+template <class M, bool PH = false, bool MH = false>
 inline void batch_rts(HostCtx<M>& ctx, const double* hx_pred, const double* hP_pred, const double* hx_filt, const double* hP_filt,
                       const double* t, int t_per_filter, double* xs, double* Ps, int T, long long B,
                       const int* quat_idxs, int n_quat, int norm_quats, void* stream,
-                      const double* x_term = nullptr, const double* P_term = nullptr, long long k0 = 0) {
+                      const double* x_term = nullptr, const double* P_term = nullptr, long long k0 = 0,
+                      const double* hP_pred_last = nullptr) {
+  static_assert(!(PH && MH), "main-block prediction histories are in the full layout");
   if (!check_packed_hist<M, PH>("batch_rts_packed")) return;
+  if constexpr (MH && M::EDIM <= 32) {
+    fprintf(stderr, "[rednose_b200] batch_rts_mainhist: main-block prediction histories exist only above EDIM 32\n");
+    last_status() = (int)cudaErrorNotSupported;
+    return;
+  }
   if (!check_quat_idxs(quat_idxs, n_quat, M::DIM)) return;
+  if (MH && B > 0 && !(x_term && P_term) && !hP_pred_last) {
+    fprintf(stderr, "[rednose_b200] batch_rts_mainhist: without a terminal estimate the newest full prediction (hP_pred_last) is required\n");
+    last_status() = (int)cudaErrorInvalidValue;
+    return;
+  }
   RtsArgs<M::NG> a;
   memset(&a, 0, sizeof(a));
   a.x_term = (x_term && P_term) ? x_term : nullptr; a.P_term = (x_term && P_term) ? P_term : nullptr; a.k0 = k0;
+  a.hP_pred_last = MH ? hP_pred_last : nullptr;
   a.hx_pred = hx_pred; a.hP_pred = hP_pred; a.hx_filt = hx_filt; a.hP_filt = hP_filt;
   a.t = t; a.t_per_filter = t_per_filter; a.xs = xs; a.Ps = Ps; a.T = T; a.B = B; a.norm_quats = norm_quats;
   a.n_quat = n_quat;
@@ -316,7 +366,8 @@ inline void batch_rts(HostCtx<M>& ctx, const double* hx_pred, const double* hP_p
                                  cudaMemcpyDeviceToDevice, (cudaStream_t)stream), "cudaMemcpyAsync(RTS P_{k|k})"))
         return;
     }
-    launch_rts_auto<M, PH>(a, (cudaStream_t)stream);
+    if constexpr (!MH) launch_rts_auto<M, PH>(a, (cudaStream_t)stream);
+    else if constexpr (M::EDIM > 32) launch_rts_auto<MainHist<M>>(a, (cudaStream_t)stream);   // refused above otherwise
   }
 }
 

@@ -25,6 +25,8 @@ enum : int {
   FLAG_AUGMENT            = 16, // MSCKF: shift the clone window after the (last) update, in the same launch (ekf_sym.py:527-528 -> :365-391); CTA kernel only
   FLAG_PACKED_P           = 32, // P is [B, packed_doubles(EDIM)] in the packed lower-block-triangle layout (ekf_packed.cuh); pair kernel only
   FLAG_PACKED_HIST        = 64, // hP_pred / hP_filt hold packed_doubles(EDIM) per filter in that layout; pair kernel only
+  FLAG_MAIN_HIST          = 128,// hP_pred holds the MEDIM x MEDIM main block per filter, hP_pred_last the full newest P_{k+1|k};
+                                // set by the <name>_batch_mainhist_step_<kind> entry points, CTA kernel (EDIM > 32) only
 };
 
 // A filter model whose covariance HISTORY slabs are packed (FLAG_PACKED_HIST, ekf_packed.cuh).  The kernels that record
@@ -40,6 +42,21 @@ template <class M>
 struct PackedHistOf<M, decltype(void(M::PACKED_HIST))> { static constexpr bool value = M::PACKED_HIST; };
 template <class M>
 constexpr bool packed_hist() { return PackedHistOf<M>::value; }
+
+// A filter model (EDIM > 32) whose PREDICTED covariance history keeps only the MEDIM x MEDIM main block per step
+// (FLAG_MAIN_HIST): the RTS recursion reads nothing else of P_{k+1|k} (ekf_sym.py:677-686).  The full newest prediction,
+// which the smoother copies to its last output row, goes to a separate [B, EDIM, EDIM] buffer.  Instantiated in place
+// of M, like PackedHist, so the full-layout kernels keep their symbols and machine code.
+template <class M>
+struct MainHist : M {
+  static constexpr bool MAIN_HIST = true;
+};
+template <class M, class = void>
+struct MainHistOf { static constexpr bool value = false; };
+template <class M>
+struct MainHistOf<M, decltype(void(M::MAIN_HIST))> { static constexpr bool value = M::MAIN_HIST; };
+template <class M>
+constexpr bool main_hist() { return MainHistOf<M>::value; }
 
 // One argument block per launch, passed by value (lives in the kernel parameter
 // constant bank: every field is warp-uniform).  NG = number of global_vars.
@@ -71,7 +88,13 @@ struct StepArgs {
   // ragged histories (gather list only): entry e records at slab element hist_row[e] * hist_B + idx[e] instead of
   // idx[e]; a negative row steps without recording.  nullptr = the slabs are indexed by filter.  Kept behind the
   // existing fields so that the launches without a gather list see the argument block they always had.
-  const int* hist_row;
+  // FLAG_MAIN_HIST, which is refused with a gather list, uses the same slot for hP_pred_last: [B, EDIM, EDIM], the full
+  // P_{k+1|k} of this step (hP_pred is then [B, MEDIM, MEDIM]).  Sharing it keeps the block's size, and so the offsets
+  // of the kernel parameters behind it, unchanged.
+  union {
+    const int* hist_row;
+    double* hP_pred_last;
+  };
   long long hist_B;      // filter stride of the history slabs
 };
 

@@ -18,6 +18,7 @@
 // through the generated sparse KIND::Herr_apply, and the projection is applied to the small ZDIM-vectors
 // (Q^T (H_err P) = (Q^T H_err) P) instead of densifying H_err.
 #pragma once
+#include <type_traits>
 #include "ekf_common.cuh"
 #include "ekf_warp.cuh"
 #include "ekf_rts_mma.cuh"   // dmma884
@@ -329,7 +330,17 @@ __global__ void __launch_bounds__(cta_threads<M>(), CTA_MIN_BLOCKS) ekf_step_cta
       }
     }
     __syncthreads();
-    if (a.hP_pred && rec) store_full(a.hP_pred + hb * (long long)(E * E));
+    if constexpr (main_hist<M>()) {
+      // main block of P_{k+1|k} into the [T, B, MEDIM, MEDIM] slab, the full matrix into the newest-prediction buffer
+      if (a.hP_pred) {
+        double* dst = a.hP_pred + hb * (long long)(ME * ME);
+        for (int i = warp; i < ME; i += nw)
+          if (lane < ME) dst[i * ME + lane] = s.Ppk[(lane <= i) ? i * (i + 1) / 2 + lane : tj[0] + i];
+      }
+      if (a.hP_pred_last) store_full(a.hP_pred_last + fb * (long long)(E * E));
+    } else {
+      if (a.hP_pred && rec) store_full(a.hP_pred + hb * (long long)(E * E));
+    }
   }
 
   if constexpr (UPD) {
@@ -537,16 +548,20 @@ __global__ void __launch_bounds__(cta_threads<M>(), CTA_MIN_BLOCKS) ekf_step_cta
   }
 }
 
-template <class M, class K, bool PRED, bool UPD, bool HIST = false>
+// MH (FLAG_MAIN_HIST): the first launch, the one that predicts, is the MainHist<M> instantiation of ekf_step_cta; the
+// leaf kernel and the update-only launches of further observations never touch hP_pred and stay M's
+template <class M, class K, bool PRED, bool UPD, bool HIST = false, bool MH = false>
 inline void launch_step_cta(const StepArgs<M::NG>& a, cudaStream_t st) {
+  static_assert(!MH || (PRED && !HIST && M::EDIM > 32), "main-block prediction histories: predicting steps above EDIM 32, no gather list");
+  using MP = std::conditional_t<MH, MainHist<M>, M>;
   using W = CtaWs<M, K>;
   // leaf-value workspace of THIS call, allocated and released in stream order (calls on different streams / devices
   // never share it)
   double* ws = (double*)stream_alloc(sizeof(double) * (size_t)a.B * W::SIZE, st, "cudaMallocAsync(cta workspace)");
   if (!ws) return;
   constexpr size_t smem = sizeof(CtaSmem<M, K>);
-  if (first_launch_of((const void*)ekf_step_cta<M, K, PRED, UPD, HIST>))
-    check(cudaFuncSetAttribute(ekf_step_cta<M, K, PRED, UPD, HIST>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem), "smem attribute");
+  if (first_launch_of((const void*)ekf_step_cta<MP, K, PRED, UPD, HIST>))
+    check(cudaFuncSetAttribute(ekf_step_cta<MP, K, PRED, UPD, HIST>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem), "smem attribute");
   if (first_launch_of((const void*)ekf_step_cta<M, K, false, UPD, HIST>))
     check(cudaFuncSetAttribute(ekf_step_cta<M, K, false, UPD, HIST>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem), "smem attribute");
   constexpr int threads = cta_threads<M>();
@@ -555,7 +570,7 @@ inline void launch_step_cta(const StepArgs<M::NG>& a, cudaStream_t st) {
     const unsigned lgrid = (unsigned)((a.B + 63) / 64);
     if (o == 0) {
       ekf_leaf_thread<M, K, PRED, UPD, HIST><<<lgrid, 64, 0, st>>>(a, o, ws);
-      ekf_step_cta<M, K, PRED, UPD, HIST><<<(unsigned)a.B, threads, smem, st>>>(a, o, ws);
+      ekf_step_cta<MP, K, PRED, UPD, HIST><<<(unsigned)a.B, threads, smem, st>>>(a, o, ws);
     } else {
       ekf_leaf_thread<M, K, false, UPD, HIST><<<lgrid, 64, 0, st>>>(a, o, ws);
       ekf_step_cta<M, K, false, UPD, HIST><<<(unsigned)a.B, threads, smem, st>>>(a, o, ws);

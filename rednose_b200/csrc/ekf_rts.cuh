@@ -65,6 +65,9 @@ struct RtsArgs {
   // ragged histories: filter b smooths rows 0 .. len[b] - 1 only (with t [T, B]) and leaves its rows >= len[b] of xs / Ps
   // untouched; nullptr = every filter has T rows.  Not combined with segment continuation.
   const int* len;
+  // M = MainHist<model> (EDIM > 32): hP_pred is [T, B, MEDIM, MEDIM], the main block of each P_{k|k-1}, and the recursion
+  // starts (without x_term / P_term) from this [B, EDIM, EDIM] full P_{T-1|T-2}
+  const double* hP_pred_last;
 };
 
 // rows filter b smooths: T, or len[b] clamped to [0, T] for a ragged history
@@ -111,13 +114,15 @@ struct RtsScratch {
 template <class M, bool RAGGED = false>
 __global__ void __launch_bounds__(RTS_WARPS * 32, RTS_MIN_CTAS) ekf_rts_warp(const RtsArgs<M::NG> a) {
   constexpr int D = M::DIM, E = M::EDIM, N = M::MEDIM, D1 = M::DMAIN;
-  constexpr bool PH = packed_hist<M>();
+  constexpr bool PH = packed_hist<M>(), MH = main_hist<M>();
   using SC = RtsScratch<M>;
   constexpr int LD = SC::LD;
   static_assert(N <= 32, "warp-per-filter RTS needs MEDIM <= 32");
   static_assert(E <= 32 || (!PH && !RAGGED), "above EDIM 32 only whole and segment histories in the full layout");
   static_assert(!PH || E % 2 == 0, "the packed layout needs an even EDIM");
+  static_assert(!MH || E > 32, "main-block prediction histories exist only above EDIM 32");
   constexpr int PS = PH ? packed_doubles(E) : E * E;   // doubles of one filter's covariance in the slabs
+  constexpr int PPS = MH ? N * N : PS, PLD = MH ? N : E;   // the same, and the row stride, in the hP_pred slab
   __shared__ SC s_all[RTS_WARPS];
   const int lane = threadIdx.x & 31, wib = threadIdx.x >> 5;
   const long long b = (long long)blockIdx.x * RTS_WARPS + wib;
@@ -128,7 +133,7 @@ __global__ void __launch_bounds__(RTS_WARPS * 32, RTS_MIN_CTAS) ekf_rts_warp(con
   const bool act = lane < N;        // owns a column of the main block
   const bool actE = lane < E;       // owns a column of the full covariance
   const int col = actE ? lane : 0;
-  const long long BP = a.B * (long long)PS, BX = a.B * (long long)D;
+  const long long BP = a.B * (long long)PS, BPP = a.B * (long long)PPS, BX = a.B * (long long)D;
 
   auto normalize_xn = [&]() {
     for (int q = 0; q < a.n_quat; ++q) {
@@ -152,7 +157,8 @@ __global__ void __launch_bounds__(RTS_WARPS * 32, RTS_MIN_CTAS) ekf_rts_warp(con
       for (int i = 0; i < N; ++i) pn[i] = Pg[packed_index(i, col)];
       if (!seg) for (int t = lane; t < PS; t += 32) Po[t] = Pg[t];
     } else if constexpr (E > 32) {
-      const double* Pg = seg ? a.P_term + b * (long long)(E * E) : a.hP_pred + k * BP + b * (long long)(E * E);
+      const double* Pg = seg ? a.P_term + b * (long long)(E * E)
+                             : (MH ? a.hP_pred_last + b * (long long)(E * E) : a.hP_pred + k * BP + b * (long long)(E * E));
       double* Po = a.Ps + k * BP + b * (long long)(E * E);
 #pragma unroll
       for (int i = 0; i < N; ++i) pn[i] = act ? Pg[i * E + lane] : 0.0;
@@ -178,12 +184,12 @@ __global__ void __launch_bounds__(RTS_WARPS * 32, RTS_MIN_CTAS) ekf_rts_warp(con
 #pragma unroll 1
   for (long long k = T - 2; k >= 0; --k) {
     const double* Pf_b = a.hP_filt + k * BP + b * (long long)PS;
-    const double* Pp_b = a.hP_pred + (k + 1) * BP + b * (long long)PS;
+    const double* Pp_b = a.hP_pred + (k + 1) * BPP + b * (long long)PPS;
     const double* Pf_g = Pf_b + col;
     const double* Pp_g = Pp_b + col;
-    // element i of the lane's column of a covariance: P is defined by its lower triangle
-    auto el = [&](const double* Pb, const double* Pg, int i) {
-      if constexpr (E > 32) return act ? Pg[i * E] : 0.0;   // main block only
+    // element i of the lane's column of a covariance (row stride ld): P is defined by its lower triangle
+    auto el = [&](const double* Pb, const double* Pg, int i, int ld = M::EDIM) {
+      if constexpr (E > 32) return act ? Pg[i * ld] : 0.0;   // main block only
       else return PH ? Pb[packed_index(i, col)] : Pg[i * E];
     };
     double g[N];
@@ -207,7 +213,7 @@ __global__ void __launch_bounds__(RTS_WARPS * 32, RTS_MIN_CTAS) ekf_rts_warp(con
     // A = column of P_{k+1|k};  dP column = P_{k+1|N} - P_{k+1|k} (pn is dead afterwards)
     double A[N];
 #pragma unroll
-    for (int i = 0; i < N; ++i) A[i] = el(Pp_b, Pp_g, i);
+    for (int i = 0; i < N; ++i) A[i] = el(Pp_b, Pp_g, i, PLD);
     if (act) {
 #pragma unroll
       for (int i = 0; i < N; ++i) s.DP[i * LD + lane] = pn[i] - A[i];

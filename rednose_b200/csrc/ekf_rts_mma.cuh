@@ -46,12 +46,14 @@ struct RtsMmaScratch {
 template <class M, bool RAGGED = false>
 __global__ void __launch_bounds__(RTS_WARPS * 32, RTS_MIN_CTAS) ekf_rts_warp_mma(const RtsArgs<M::NG> a) {
   constexpr int D = M::DIM, E = M::EDIM, N = M::MEDIM, D1 = M::DMAIN;
-  constexpr bool PH = packed_hist<M>();
+  constexpr bool PH = packed_hist<M>(), MH = main_hist<M>();
   using SC = RtsMmaScratch<M>;
   constexpr int LD = SC::LD, NP = SC::NP, LP = SC::LP, NT = NP / 8, NK = NP / 4;
   static_assert(E % 2 == 0 && N <= 32, "fragment I/O needs an even EDIM and MEDIM <= 32");
   static_assert(E <= 32 || (!PH && !RAGGED), "above EDIM 32 only whole and segment histories in the full layout");
+  static_assert(!MH || E > 32, "main-block prediction histories exist only above EDIM 32");
   constexpr int PS = PH ? packed_doubles(E) : E * E;   // doubles of one filter's covariance in the slabs
+  constexpr int PPS = MH ? N * N : PS, PLD = MH ? N : E;   // the same, and the row stride, in the hP_pred slab
   // dynamic: from a main block of 25 (NP = 32) the RTS_WARPS scratch blocks pass the 48 KB static limit
   extern __shared__ __align__(16) unsigned char rts_smem_raw[];
   SC* s_all = reinterpret_cast<SC*>(rts_smem_raw);
@@ -64,7 +66,7 @@ __global__ void __launch_bounds__(RTS_WARPS * 32, RTS_MIN_CTAS) ekf_rts_warp_mma
   const bool act = lane < N, actE = lane < E;
   const int col = actE ? lane : 0;
   const int fg = lane >> 2, ft = lane & 3;   // fragment coordinates: row fg, k / column pair ft
-  const long long BP = a.B * (long long)PS, BX = a.B * (long long)D;
+  const long long BP = a.B * (long long)PS, BPP = a.B * (long long)PPS, BX = a.B * (long long)D;
 
   auto normalize_xn = [&]() {
     for (int q = 0; q < a.n_quat; ++q) {
@@ -77,10 +79,17 @@ __global__ void __launch_bounds__(RTS_WARPS * 32, RTS_MIN_CTAS) ekf_rts_warp_mma
   };
   // element pair (r, c), (r, c+1) of tile (mi, ni) in accumulator layout
   auto frag_rc = [&](int mi, int ni, int& r, int& c) { r = mi * 8 + fg; c = ni * 8 + 2 * ft; };
-  // elements (r, c), (r, c + 1) of the covariance at Pb
-  auto pair_at = [&](const double* Pb, int r, int c) {
+  // elements (r, c), (r, c + 1) of the covariance at Pb (row stride ld)
+  auto pair_at = [&](const double* Pb, int r, int c, int ld = M::EDIM) {
     if constexpr (PH) return packed_pair(Pb, r, c);
-    else return *reinterpret_cast<const double2*>(Pb + r * E + c);
+    else return *reinterpret_cast<const double2*>(Pb + r * ld + c);
+  };
+  // elements (r, c), (r, c + 1) of P_{k+1|k}.  A main-block slab of odd MEDIM (an even EDIM with position clones, EAUG 3)
+  // has rows of odd length: its pairs are not 16-byte aligned, and (r, MEDIM) is not in the row.  That element only
+  // meets the zero padding of X (row MEDIM), so 0 stands in for it; the products come out as from the full slab.
+  auto pred_pair = [&](const double* Pb, int r, int c) {
+    if constexpr (MH && N % 2 == 1) return make_double2(Pb[r * N + c], c + 1 < N ? Pb[r * N + c + 1] : 0.0);
+    else return pair_at(Pb, r, c, PLD);
   };
 
   // ---- start: smoothed = predicted at T-1 (ekf_sym.py:658-659); carried in fragment layout ----
@@ -88,7 +97,8 @@ __global__ void __launch_bounds__(RTS_WARPS * 32, RTS_MIN_CTAS) ekf_rts_warp_mma
   {
     const long long k = T - 1;
     const bool seg = a.x_term != nullptr;   // segment continuation: start from the smoothed estimate handed in
-    const double* Pg = seg ? a.P_term + b * (long long)PS : a.hP_pred + k * BP + b * (long long)PS;
+    const double* Pg = seg ? a.P_term + b * (long long)PS
+                           : (MH ? a.hP_pred_last + b * (long long)PS : a.hP_pred + k * BP + b * (long long)PS);
     double* Po = a.Ps + k * BP + b * (long long)PS;
     if (!seg) for (int idx = lane; idx < PS; idx += 32) Po[idx] = Pg[idx];
 #pragma unroll
@@ -111,7 +121,7 @@ __global__ void __launch_bounds__(RTS_WARPS * 32, RTS_MIN_CTAS) ekf_rts_warp_mma
 #pragma unroll 1
   for (long long k = T - 2; k >= 0; --k) {
     const double* Pf_b = a.hP_filt + k * BP + b * (long long)PS;
-    const double* Pp_b = a.hP_pred + (k + 1) * BP + b * (long long)PS;
+    const double* Pp_b = a.hP_pred + (k + 1) * BPP + b * (long long)PPS;
     const double* Pf_g = Pf_b + col;
     const double* Pp_g = Pp_b + col;
     // every global load of the step is issued here, before any dependent work (one latency round trip per step)
@@ -119,7 +129,7 @@ __global__ void __launch_bounds__(RTS_WARPS * 32, RTS_MIN_CTAS) ekf_rts_warp_mma
 #pragma unroll
     for (int i = 0; i < N; ++i) {
       if constexpr (PH) { g[i] = Pf_b[packed_index(i, col)]; A[i] = Pp_b[packed_index(i, col)]; }   // lower triangle
-      else if constexpr (E > 32) { g[i] = act ? Pf_g[i * E] : 0.0; A[i] = act ? Pp_g[i * E] : 0.0; }   // main block only
+      else if constexpr (E > 32) { g[i] = act ? Pf_g[i * E] : 0.0; A[i] = act ? Pp_g[i * PLD] : 0.0; }   // main block only
       else { g[i] = Pf_g[i * E]; A[i] = Pp_g[i * E]; }
     }
     // P_{k|k} once more, in accumulator layout (the C operand of the last product): fetched here with everything
@@ -144,7 +154,7 @@ __global__ void __launch_bounds__(RTS_WARPS * 32, RTS_MIN_CTAS) ekf_rts_warp_mma
       };
       if (k > 0 && act) {
         prefetch_row(Pf_b - BP + lane * E);
-        prefetch_row(a.hP_pred + k * BP + b * (long long)PS + lane * E);
+        prefetch_row(a.hP_pred + k * BPP + b * (long long)PPS + lane * PLD);
       }
       if (k > 0 && lane < (D - 1) / 16 + 2) {   // x rows likewise: points at most 16 doubles apart, the last one included
         const int xo = lane * 16 < D ? lane * 16 : D - 1;
@@ -171,7 +181,7 @@ __global__ void __launch_bounds__(RTS_WARPS * 32, RTS_MIN_CTAS) ekf_rts_warp_mma
         int r, c; frag_rc(mi, ni, r, c);
         double2 v = make_double2(0.0, 0.0);
         if (r < N && c < N) {
-          const double2 pp = pair_at(Pp_b, r, c);
+          const double2 pp = pred_pair(Pp_b, r, c);
           v.x = pn[(mi * NT + ni) * 2] - pp.x;
           v.y = pn[(mi * NT + ni) * 2 + 1] - pp.y;
         }

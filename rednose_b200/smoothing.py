@@ -11,22 +11,32 @@ Both smoothers take ``packed_history=True`` for filters with a packed covariance
 packed=True)): the history then stores each covariance as its packed lower block triangle (4 592 instead of 8 112 bytes
 per live filter-step, so 1.77x the filters per tile), and the sink receives the smoothed covariances packed,
 [..., packed doubles]; ``unpack_P`` turns them into full matrices.
+
+For an MSCKF (EDIM > 32), ``main_pred=True`` keeps only the main block of each predicted covariance in the history
+(BatchedEKF.new_history(T, main_pred=True)): the smoother reads nothing else of it.  A msckf step then takes 59 152
+instead of 109 072 bytes; the smoothed covariances stay full and bit-identical.
+
+``obs_fn(k, lo, hi)`` returns ``(t, kind, z, R)`` or ``(t, kind, z, R, ea, augment)``: ``ea`` are the extra arguments of
+the kind (the triangulated landmark of a feature-track kind, [hi - lo, EADIM] or None) and ``augment`` shifts the MSCKF
+clone window after the update (predict_and_update_batch(..., augment=True)).
 """
 from __future__ import annotations
 
 import torch
 
-from rednose_b200.batched import PACKED_REFUSED, BatchedEKF, packed_P_doubles
+from rednose_b200.batched import MAIN_PRED_REFUSED, PACKED_REFUSED, BatchedEKF, main_pred_doubles, packed_P_doubles
 
 
-def history_bytes_per_filter(dim_x, dim_err, T, smoothed_in_place=True, packed_doubles=0):
+def history_bytes_per_filter(dim_x, dim_err, T, smoothed_in_place=True, packed_doubles=0, main_pred_doubles=0):
   """Bytes of a T-step history of one filter; packed_doubles > 0: its covariances are in the packed layout of that many
-  doubles (BatchedEKF.new_history(T, packed=True))."""
+  doubles (BatchedEKF.new_history(T, packed=True)); main_pred_doubles > 0: its predicted covariances keep only their
+  main block of that many doubles, plus one full copy of the newest prediction (BatchedEKF.new_history(T,
+  main_pred=True))."""
   cov = packed_doubles or dim_err * dim_err
-  per_step = 2 * cov + 2 * dim_x
+  per_step = cov + (main_pred_doubles or cov) + 2 * dim_x
   if not smoothed_in_place:
     per_step += cov + dim_x
-  return 8 * per_step * T
+  return 8 * per_step * T + (8 * dim_err * dim_err if main_pred_doubles else 0)
 
 
 def _history_doubles(folder, name, packed_history):
@@ -38,18 +48,36 @@ def _history_doubles(folder, name, packed_history):
   return pd
 
 
+def _main_pred_doubles(folder, name, main_pred, packed_history):
+  if not main_pred:
+    return 0
+  if packed_history:
+    raise ValueError("a main-block prediction history is in the full covariance layout: packed_history does not apply")
+  md = main_pred_doubles(folder, name)
+  if not md:
+    raise ValueError(f"filter '{name}': {MAIN_PRED_REFUSED}")
+  return md
+
+
+def _observation(obs_fn, k, lo, hi):
+  """(t, kind, z, R, ea, augment) of step k: obs_fn returns the first four, or all six."""
+  obs = obs_fn(k, lo, hi)
+  return tuple(obs) if len(obs) == 6 else (*obs, None, False)
+
+
 class TiledSmoother:
   """Forward filter + RTS smoother, one tile of filters with its whole history at a time.  With packed_history=True the
   history and the smoothed covariances the sink receives are packed [T, n, packed doubles]; unpack_P(Ps) gives them full."""
 
   def __init__(self, folder, name, Q, dim_x, dim_err, quaternion_idxs=(), device="cuda", hbm_budget_bytes=60 << 30, tile=None,
-               packed_history=False):
+               packed_history=False, main_pred=False):
     self.folder, self.name, self.Q = folder, name, Q
     self.dim_x, self.dim_err = dim_x, dim_err
     self.quat = tuple(quaternion_idxs)
     self.device = torch.device(device)
     self.budget = hbm_budget_bytes
     self.tile = tile
+    self.main_pred_doubles = _main_pred_doubles(folder, name, main_pred, packed_history)
     self.packed_doubles = _history_doubles(folder, name, packed_history)
     self._engine = None
     self._hist = None
@@ -57,7 +85,8 @@ class TiledSmoother:
   def tile_size(self, T):
     if self.tile:
       return self.tile
-    per = history_bytes_per_filter(self.dim_x, self.dim_err, T, packed_doubles=self.packed_doubles) + 8 * (self.dim_err**2 + self.dim_x)
+    per = history_bytes_per_filter(self.dim_x, self.dim_err, T, packed_doubles=self.packed_doubles,
+                                   main_pred_doubles=self.main_pred_doubles) + 8 * (self.dim_err**2 + self.dim_x)
     return max(1, int(self.budget // per))
 
   def unpack_P(self, Ps):
@@ -65,8 +94,8 @@ class TiledSmoother:
     return self._engine.unpack_P(Ps)
 
   def run(self, x0, P0, T, obs_fn, sink, norm_quats=False, t0=0.0, passes=1):
-    """x0 [B, DIM], P0 [B, EDIM, EDIM] (host or device).  obs_fn(k, lo, hi) -> (t, kind, z [hi-lo, m], R) gives the
-    observation of step k for filters lo..hi.  sink(lo, hi, xs [T, n, DIM], Ps [T, n, EDIM, EDIM], or [T, n, packed
+    """x0 [B, DIM], P0 [B, EDIM, EDIM] (host or device).  obs_fn(k, lo, hi) -> (t, kind, z [hi-lo, m], R) or (t, kind, z,
+    R, ea, augment) gives the observation of step k for filters lo..hi.  sink(lo, hi, xs [T, n, DIM], Ps [T, n, EDIM, EDIM], or [T, n, packed
     doubles] with packed_history) receives device views that are only valid during the call.  Returns the number of
     tiles.
 
@@ -81,7 +110,8 @@ class TiledSmoother:
       n = hi - lo
       if self._engine is None or self._engine.B != n:
         self._engine = BatchedEKF(self.folder, self.name, self.Q, x0[lo:hi], P0[lo:hi], device=self.device, quaternion_idxs=self.quat)
-        self._hist = self._engine.new_history(T, packed=bool(self.packed_doubles)) if (self._hist is None or self._hist.B != n or self._hist.T != T) else self._hist
+        self._hist = (self._engine.new_history(T, packed=bool(self.packed_doubles), main_pred=bool(self.main_pred_doubles))
+                      if (self._hist is None or self._hist.B != n or self._hist.T != T) else self._hist)
       else:
         self._engine.init_state(x0[lo:hi], P0[lo:hi], None)
       eng, hist = self._engine, self._hist
@@ -91,8 +121,8 @@ class TiledSmoother:
         hist.n = 0
         eng.filter_time = t0
         for k in range(T):
-          t, kind, z, R = obs_fn(k, lo, hi)
-          eng.step_recorded(hist, kind, t, z, R)
+          t, kind, z, R, ea, aug = _observation(obs_fn, k, lo, hi)
+          eng.step_recorded(hist, kind, t, z, R, ea, augment=aug)
         xs, Ps = eng.rts_smooth(hist, norm_quats=norm_quats, quaternion_idxs=self.quat or (3,), in_place=True)
       sink(lo, hi, xs, Ps)
       tiles += 1
@@ -113,15 +143,19 @@ class CheckpointedSmoother:
   whole history at once (tests/test_parity_gpu.py::test_checkpointed_smoother_equals_full_history).
 
   packed_history=True: the segment history, the smoothed estimate handed between segments and the covariances the sink
-  receives are packed ([..., packed doubles]; unpack_P gives them full); the checkpoints stay full."""
+  receives are packed ([..., packed doubles]; unpack_P gives them full); the checkpoints stay full.
+
+  main_pred=True (EDIM > 32): the segment history keeps the main block of each predicted covariance only (see the module
+  docstring); checkpoints, the estimate handed between segments and the sink's covariances stay full."""
 
   def __init__(self, folder, name, Q, dim_x, dim_err, quaternion_idxs=(), device="cuda", hbm_budget_bytes=60 << 30, segment=64, tile=None,
-               packed_history=False):
+               packed_history=False, main_pred=False):
     self.folder, self.name, self.Q = folder, name, Q
     self.dim_x, self.dim_err = dim_x, dim_err
     self.quat = tuple(quaternion_idxs)
     self.device = torch.device(device)
     self.budget, self.segment, self.tile = hbm_budget_bytes, int(segment), tile
+    self.main_pred_doubles = _main_pred_doubles(folder, name, main_pred, packed_history)
     self.packed_doubles = _history_doubles(folder, name, packed_history)
     self._engine = self._hist = self._ck = None
     self.stats = {}
@@ -129,7 +163,8 @@ class CheckpointedSmoother:
   def bytes_per_filter(self, T):
     nseg = (T + self.segment - 1) // self.segment
     state = 8 * (self.dim_err**2 + self.dim_x)
-    return nseg * state + history_bytes_per_filter(self.dim_x, self.dim_err, self.segment + 1, packed_doubles=self.packed_doubles) + 3 * state
+    return nseg * state + history_bytes_per_filter(self.dim_x, self.dim_err, self.segment + 1, packed_doubles=self.packed_doubles,
+                                                   main_pred_doubles=self.main_pred_doubles) + 3 * state
 
   def unpack_P(self, Ps):
     """Full [..., EDIM, EDIM] covariances of packed smoothed ones (the sink's Ps with packed_history=True)."""
@@ -146,8 +181,8 @@ class CheckpointedSmoother:
     return (B + ntiles - 1) // ntiles, ntiles
 
   def run(self, x0, P0, T, obs_fn, sink, norm_quats=False, t0=0.0):
-    """obs_fn(k, lo, hi) -> (t, kind, z, R) must return the SAME observation every time it is asked for step k (each step
-    is filtered twice) in a buffer the kernel may overwrite.  sink(lo, hi, k0, xs [n, tile, DIM], Ps [n, tile, EDIM, EDIM])
+    """obs_fn(k, lo, hi) -> (t, kind, z, R) or (t, kind, z, R, ea, augment) must return the SAME observation every time it
+    is asked for step k (each step is filtered twice) in a buffer the kernel may overwrite.  sink(lo, hi, k0, xs [n, tile, DIM], Ps [n, tile, EDIM, EDIM])
     receives the smoothed steps k0 .. k0 + n - 1 of filters lo..hi (segments arrive last to first; views valid during
     the call only; Ps [n, tile, packed doubles] with packed_history).  Returns the number of tiles."""
     B, S = x0.shape[0], self.segment
@@ -162,7 +197,7 @@ class CheckpointedSmoother:
       if self._engine is None or self._engine.B != n:
         self._engine = self._hist = self._ck = self._term = None   # release the previous tile's buffers before allocating
         self._engine = BatchedEKF(self.folder, self.name, self.Q, x0[lo:hi], P0[lo:hi], device=self.device, quaternion_idxs=self.quat)
-        self._hist = self._engine.new_history(S + 1, packed=bool(self.packed_doubles))
+        self._hist = self._engine.new_history(S + 1, packed=bool(self.packed_doubles), main_pred=bool(self.main_pred_doubles))
         self._ck = (torch.empty(nseg, n, self.dim_x, dtype=torch.float64, device=self.device),
                     torch.empty(nseg, n, self.dim_err, self.dim_err, dtype=torch.float64, device=self.device))
         self._term = (torch.empty(n, self.dim_x, dtype=torch.float64, device=self.device),
@@ -181,8 +216,8 @@ class CheckpointedSmoother:
       for k in range(T):
         if k % S == 0:
           ck_x[k // S].copy_(eng.x); ck_P[k // S].copy_(eng.P); ck_t[k // S] = eng.filter_time
-        t, kind, z, R = obs_fn(k, lo, hi)
-        eng.predict_and_update_batch(t, kind, z, R)
+        t, kind, z, R, ea, aug = _observation(obs_fn, k, lo, hi)
+        eng.predict_and_update_batch(t, kind, z, R, ea, augment=aug)
       ev[1].record(); ev[1].synchronize(); fwd_ms += ev[0].elapsed_time(ev[1])
       # ---- pass 2: segments last to first: forward with history from the checkpoint, then backward ----
       have_term = False
@@ -193,8 +228,8 @@ class CheckpointedSmoother:
         hist.n = 0
         ev[0].record()
         for k in range(k0, k1):
-          t, kind, z, R = obs_fn(k, lo, hi)
-          eng.step_recorded(hist, kind, t, z, R)
+          t, kind, z, R, ea, aug = _observation(obs_fn, k, lo, hi)
+          eng.step_recorded(hist, kind, t, z, R, ea, augment=aug)
         ev[1].record(); ev[1].synchronize(); refwd_ms += ev[0].elapsed_time(ev[1])
         ev[0].record()
         xs, Ps = eng.rts_smooth(hist, norm_quats=norm_quats, quaternion_idxs=self.quat or (3,), in_place=True,
