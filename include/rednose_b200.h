@@ -22,6 +22,9 @@
  *         row hist_row[e] (negative: not recorded) of [T, hist_B, ...] history slabs
  *     int <name>_batch_rts_ragged(...)   filter b smooths rows 0 .. len[b] - 1 with its times t [T, B]; rows >= len[b]
  *         of xs / Ps are left as they are.  EDIM <= 32 only (cudaErrorNotSupported otherwise)
+ *     int <name>_batch_restore_hist(...)   filter idx[e] of the resident x / P <- row hist_row[e] (negative: skipped) of
+ *         the x_filt / P_filt slabs, the estimate that row recorded (a rewind to it).  REDNOSE_PACKED_HIST gives the slabs'
+ *         layout, REDNOSE_PACKED_P the resident one, any pair of them.  EDIM <= 32 only (cudaErrorNotSupported otherwise)
  *   batched, HOST pointers (copies inside): <name>_host_step_<kind>(...)
  *   packed covariance layout (int results, so the reference's `void ` prototype set is unchanged):
  *     int <name>_packed_P_doubles(void)   doubles per filter of the packed layout, 0 where it is not used
@@ -74,6 +77,8 @@ typedef void (*rednose_batch_rts_fn)(const double *hx_pred, const double *hP_pre
 typedef int (*rednose_batch_step_hist_idx_fn)(double *x, double *P, const double *Q, const double *dt_arr, double dt, double *z, const double *R, const double *ea, int n_obs, long long B, const int *quat_idxs, int n_quat, int flags, double *hx_pred, double *hP_pred, double *hx_filt, double *hP_filt, const int *idx, const int *hist_row, long long hist_B, void *stream);
 /* ragged histories: filter b smooths its first len[b] of T rows, times t [T, B] */
 typedef int (*rednose_batch_rts_ragged_fn)(const double *hx_pred, const double *hP_pred, const double *hx_filt, const double *hP_filt, const double *t, const int *len, double *xs, double *Ps, int T, long long B, const int *quat_idxs, int n_quat, int norm_quats, void *stream);
+/* ragged histories: filter idx[e] of the resident x / P <- slab element hist_row[e] * hist_B + idx[e] of hx_filt / hP_filt */
+typedef int (*rednose_batch_restore_hist_fn)(const double *hx_filt, const double *hP_filt, const int *idx, const int *hist_row, long long n, long long hist_B, double *x, double *P, int flags, void *stream);
 
 /* Plugin descriptor: replaces `struct EKF` (ekf.h:16-33).  Arrays have n_kinds entries,
  * parallel to `kinds`. */

@@ -465,6 +465,22 @@ class BatchedEKF:
     row k of filter b is the k-th step that filter recorded.  packed: as in new_history."""
     return RaggedHistory(T, self.B, self.dim_x, self.dim_err, self.device, self._history_doubles(packed))
 
+  def restore_from_history(self, hist, ids, rows):
+    """Set x and P of the filters `ids` ([m] distinct) to x_filt / P_filt of row rows[e] ([m] int32) of the RaggedHistory
+    `hist`: the estimate filter ids[e] recorded there.  One launch; an entry with a negative row is skipped."""
+    ids = torch.as_tensor(ids, device=self.device).to(torch.int32).contiguous()
+    rows = torch.as_tensor(rows, device=self.device).to(torch.int32).contiguous()
+    assert hist.B == self.B and ids.shape == rows.shape, (hist.B, self.B, tuple(ids.shape), tuple(rows.shape))
+    hflag = self._hist_flag(hist.P_filt)
+    P, pflag = self._P_arg()
+    with torch.cuda.device(self.device):
+      getattr(self._lib, f"{self.name}_batch_restore_hist")(
+        self._cp(hist.x_filt), self._cp(hist.P_filt), self._ffi.cast("const int *", ids.data_ptr()),
+        self._ffi.cast("const int *", rows.data_ptr()), int(ids.shape[0]), hist.B, self._p(self.x), P, pflag | hflag,
+        self._stream())
+    self.launches += 1
+    self._check("batch_restore_hist")
+
   def step_recorded(self, hist, kind, t, z, R, ea=None, augment=False):
     """predict_and_update_batch that also appends this step to `hist` (the kernel writes the slabs itself).  augment=True
     shifts the MSCKF clone window after the update, as step(augment=True); the recorded x_{k|k} / P_{k|k} are the
@@ -640,6 +656,13 @@ class RaggedHistory:
     self.n[ids] = k + (~full).to(torch.int32)
     self.overflow += full.sum()
     return torch.where(full, -1, k).to(torch.int32)
+
+  def rewind(self, ids, rows):
+    """Make row rows[e] the newest row of filter ids[e] (distinct): n[ids] = rows + 1.  The rows above are stale and are
+    overwritten as the filter records again; the smoother never reads them.  `overflow` is left as it is."""
+    dev = self.n.device
+    ids = torch.as_tensor(ids, device=dev).to(torch.int64)
+    self.n[ids] = torch.as_tensor(rows, device=dev).to(torch.int32) + 1
 
   def overflowed(self):
     """Steps not recorded because their filter's rows were used up (synchronises with the device)."""

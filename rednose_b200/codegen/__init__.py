@@ -381,6 +381,11 @@ def gen_code(folder, name, f_sym, dt_sym, x_sym, obs_eqs, dim_x, dim_err, eskf_p
                              ("rts_ragged", brr, f"batch_rts_ragged<{model}, true>(ctx_(), hx_pred, hP_pred, hx_filt, hP_filt, t, len, xs, Ps, T, B, quat_idxs, n_quat, norm_quats, stream)")):
     hdr.append(f"int {name}_batch_{suffix}_packed({args});")
     c.append(f'extern "C" int {name}_batch_{suffix}_packed({args}) {{ return rnb::call_status([&] {{ rnb::{call}; }}); }}\n')
+  # restore filters idx[e] of the resident x / P from row hist_row[e] of a ragged history's x_filt / P_filt slabs (a
+  # rewind); flags: REDNOSE_PACKED_HIST / REDNOSE_PACKED_P give the two layouts.  int result (see _hist_idx)
+  rh = "const double *hx_filt, const double *hP_filt, const int *idx, const int *hist_row, long long n, long long hist_B, double *x, double *P, int flags, void *stream"
+  hdr.append(f"int {name}_batch_restore_hist({rh});")
+  c.append(f'extern "C" int {name}_batch_restore_hist({rh}) {{ return rnb::call_status([&] {{ rnb::batch_restore_hist<{model}>(hx_filt, hP_filt, idx, hist_row, n, hist_B, x, P, flags, stream); }}); }}\n')
   # doubles per filter and step of a main-block prediction history (MEDIM^2), 0 where it does not exist (EDIM <= 32)
   hdr.append(f"int {name}_main_pred_doubles(void);")
   c.append(f'extern "C" int {name}_main_pred_doubles(void) {{ return {MEDIM * MEDIM if EDIM > 32 else 0}; }}\n')

@@ -436,6 +436,71 @@ inline int convert_P(double* full, double* packed, const int* idx, long long n, 
   }
 }
 
+// ------------------------------------------------------ restore filters from history rows ---
+// Filter idx[e] of the resident x [*, D] / P <- slab element hist_row[e] * hist_B + idx[e] of hx_filt / hP_filt (the
+// addressing of the recording steps, hist_slot); an entry with a negative row is skipped.  PH: the history covariances
+// are packed, PP: the resident P is.  One thread per destination double.  Across layouts the copy is the one convert_P
+// makes: into the packed layout from the lower triangle, out of it as the exact mirror.
+template <int D, int E, bool PH, bool PP>
+__global__ void __launch_bounds__(256) restore_hist_kernel(const double* __restrict__ hx, const double* __restrict__ hP,
+                                                           const int* __restrict__ idx, const int* __restrict__ hist_row,
+                                                           long long n, long long hist_B, double* __restrict__ x, double* __restrict__ P) {
+  constexpr int SH = PH ? packed_doubles(E) : E * E, SP = PP ? packed_doubles(E) : E * E, W = D + SP;
+  const long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (t >= n * W) return;
+  const long long e = t / W;
+  const int r = hist_row[e];
+  if (r < 0) return;
+  const long long f = idx[e], s = (long long)r * hist_B + f;
+  const int c = (int)(t - e * W);
+  if (c < D) {
+    x[f * D + c] = hx[s * D + c];
+    return;
+  }
+  const int k = c - D;
+  int src = k;
+  if constexpr (PP && !PH) {
+    int i, j;
+    packed_element(E, k, i, j);
+    src = i >= j ? i * E + j : j * E + i;
+  } else if constexpr (PH && !PP) {
+    src = packed_index(k / E, k % E);
+  }
+  P[f * SP + k] = hP[s * SH + src];
+}
+
+template <class M>
+inline void batch_restore_hist(const double* hx_filt, const double* hP_filt, const int* idx, const int* hist_row, long long n,
+                               long long hist_B, double* x, double* P, int flags, void* stream) {
+  if (!check_packed_flag<M, false>(flags, "batch_restore_hist")) return;
+  if constexpr (M::EDIM > 32) {
+    fprintf(stderr, "[rednose_b200] batch_restore_hist: ragged histories exist only up to EDIM 32 (EDIM = %d)\n", M::EDIM);
+    last_status() = (int)cudaErrorNotSupported;
+  } else {
+    if (n < 0 || hist_B <= 0 || (n > 0 && (!hx_filt || !hP_filt || !idx || !hist_row || !x || !P))) {
+      fprintf(stderr, "[rednose_b200] batch_restore_hist: n >= 0, a positive slab stride and, for n > 0, every pointer are required\n");
+      last_status() = (int)cudaErrorInvalidValue;
+      return;
+    }
+    if (n == 0) return;
+    constexpr int D = M::DIM, E = M::EDIM;
+    const bool ph = flags & FLAG_PACKED_HIST, pp = flags & FLAG_PACKED_P;
+    auto run = [&](auto kern, int w) {
+      kern<<<(unsigned)((n * w + 255) / 256), 256, 0, (cudaStream_t)stream>>>(hx_filt, hP_filt, idx, hist_row, n, hist_B, x, P);
+    };
+    if constexpr (pair_may_serve<M>()) {
+      constexpr int PD = packed_doubles(E);
+      if (ph && pp) run(restore_hist_kernel<D, E, true, true>, D + PD);
+      else if (ph) run(restore_hist_kernel<D, E, true, false>, D + E * E);
+      else if (pp) run(restore_hist_kernel<D, E, false, true>, D + PD);
+      else run(restore_hist_kernel<D, E, false, false>, D + E * E);
+    } else {
+      run(restore_hist_kernel<D, E, false, false>, D + E * E);   // check_packed_flag refused the packed flags
+    }
+    check(cudaGetLastError(), "batch_restore_hist launch");
+  }
+}
+
 // --------------------------------------------- batched, HOST buffers (stateless) ---
 // Full round trip: x,P,z,R(,ea) host -> device, fused step, x,P,y device -> host, in
 // chunks on alternating streams so copies overlap the kernel when the host
