@@ -22,6 +22,13 @@
  *         row hist_row[e] (negative: not recorded) of [T, hist_B, ...] history slabs
  *     int <name>_batch_rts_ragged(...)   filter b smooths rows 0 .. len[b] - 1 with its times t [T, B]; rows >= len[b]
  *         of xs / Ps are left as they are.  EDIM <= 32 only (cudaErrorNotSupported otherwise)
+ *     int <name>_batch_rts_ragged_segment(...)   one segment of a stream too long for one history: as _batch_rts_ragged,
+ *         with k0[b] the global index of filter b's row 0 (quaternions are normalised in every output but global row 0).
+ *         term[b] != 0: row len[b] - 1 is the first row of the filter's segment behind, read for its predicted state and
+ *         time only; the recursion starts from x_term[b] [DIM] / P_term[b], that row's smoothed estimate, and row len[b] - 1
+ *         of xs / Ps is not written.  term[b] == 0: the filter is smoothed as by _batch_rts_ragged.  packed != 0: every
+ *         covariance slab and P_term are packed (cudaErrorNotSupported where <name>_packed_P_doubles() is 0).  B = 0
+ *         launches nothing.  EDIM <= 32 only (cudaErrorNotSupported otherwise)
  *     int <name>_batch_restore_hist(...)   filter idx[e] of the resident x / P <- row hist_row[e] (negative: skipped) of
  *         the x_filt / P_filt slabs, the estimate that row recorded (a rewind to it).  REDNOSE_PACKED_HIST gives the slabs'
  *         layout, REDNOSE_PACKED_P the resident one, any pair of them.  EDIM <= 32 only (cudaErrorNotSupported otherwise)
@@ -77,6 +84,9 @@ typedef void (*rednose_batch_rts_fn)(const double *hx_pred, const double *hP_pre
 typedef int (*rednose_batch_step_hist_idx_fn)(double *x, double *P, const double *Q, const double *dt_arr, double dt, double *z, const double *R, const double *ea, int n_obs, long long B, const int *quat_idxs, int n_quat, int flags, double *hx_pred, double *hP_pred, double *hx_filt, double *hP_filt, const int *idx, const int *hist_row, long long hist_B, void *stream);
 /* ragged histories: filter b smooths its first len[b] of T rows, times t [T, B] */
 typedef int (*rednose_batch_rts_ragged_fn)(const double *hx_pred, const double *hP_pred, const double *hx_filt, const double *hP_filt, const double *t, const int *len, double *xs, double *Ps, int T, long long B, const int *quat_idxs, int n_quat, int norm_quats, void *stream);
+/* ragged histories: one segment; filter b's row 0 is its global row k0[b], and with term[b] != 0 its row len[b] - 1 is
+   the first row of its segment behind, smoothed to (x_term[b], P_term[b]); packed != 0: packed covariance slabs */
+typedef int (*rednose_batch_rts_ragged_segment_fn)(const double *hx_pred, const double *hP_pred, const double *hx_filt, const double *hP_filt, const double *t, const int *len, const unsigned char *term, const long long *k0, const double *x_term, const double *P_term, double *xs, double *Ps, int T, long long B, const int *quat_idxs, int n_quat, int norm_quats, int packed, void *stream);
 /* ragged histories: filter idx[e] of the resident x / P <- slab element hist_row[e] * hist_B + idx[e] of hx_filt / hP_filt */
 typedef int (*rednose_batch_restore_hist_fn)(const double *hx_filt, const double *hP_filt, const int *idx, const int *hist_row, long long n, long long hist_B, double *x, double *P, int flags, void *stream);
 

@@ -572,6 +572,46 @@ class BatchedEKF:
     self._check("batch_rts_ragged")
     return xs, Ps
 
+  def rts_smooth_ragged_segment(self, hist, term, k0, terminal, norm_quats=False, quaternion_idxs=(3,), in_place=False,
+                                out=None):
+    """RTS backward pass over one SEGMENT of per-filter streams too long for one RaggedHistory (RaggedCheckpointedSmoother
+    in rednose_b200/smoothing.py drives it).  Filter b's n[b] rows of `hist` are its global rows k0[b] .. k0[b] + n[b] - 1
+    (k0 [B] int64): every smoothed state but that of global row 0 has its quaternions normalised, as in a whole pass.
+
+    term [B] (bool or uint8): where set, filter b's last row (n[b] - 1) is the first row of its segment behind, of which only
+    the predicted state and time are read, and the recursion starts from terminal = (x [B, DIM], P [B, EDIM, EDIM], packed
+    like the history), that row's smoothed estimate; row n[b] - 1 of xs / Ps is then not written.  Elsewhere filter b is
+    smoothed as rts_smooth(hist) smooths it.  Returns (xs, Ps) [T, B, ...] like rts_smooth(hist)."""
+    lost = hist.overflowed()
+    if lost:
+      raise RuntimeError(f"ragged history overflow: {lost} step(s) found their filter's {hist.T} rows used up and were "
+                         f"not recorded; record into a longer history")
+    term = torch.as_tensor(term, device=self.device).to(torch.uint8).contiguous()
+    k0 = torch.as_tensor(k0, device=self.device).to(torch.int64).contiguous()
+    xt, Pt = terminal
+    assert term.shape == (self.B,) and k0.shape == (self.B,), (tuple(term.shape), tuple(k0.shape))
+    assert xt.is_contiguous() and Pt.is_contiguous() and xt.shape == (self.B, self.dim_x) and Pt.shape == hist.P_filt.shape[1:], \
+      "terminal=(x [B, DIM], P [B, EDIM, EDIM] or, for a packed history, [B, packed doubles])"
+    if out is not None:
+      xs, Ps = out
+      assert xs.shape == hist.x_filt.shape and Ps.shape == hist.P_filt.shape and xs.is_contiguous() and Ps.is_contiguous()
+    elif in_place:
+      xs, Ps = hist.x_filt, hist.P_filt
+    else:
+      xs = torch.full_like(hist.x_filt, float("nan"))
+      Ps = torch.full_like(hist.P_filt, float("nan"))
+    qi = self._ffi.new("int[]", list(quaternion_idxs) or [0])
+    with torch.cuda.device(self.device):
+      getattr(self._lib, f"{self.name}_batch_rts_ragged_segment")(
+        self._cp(hist.x_pred), self._cp(hist.P_pred), self._cp(hist.x_filt), self._cp(hist.P_filt), self._cp(hist.t),
+        self._ffi.cast("const int *", hist.n.data_ptr()), self._ffi.cast("const unsigned char *", term.data_ptr()),
+        self._ffi.cast("const long long *", k0.data_ptr()), self._cp(xt), self._cp(Pt), self._p(xs), self._p(Ps), hist.T,
+        self.B, qi, len(quaternion_idxs) if norm_quats else 0, 1 if norm_quats else 0, 1 if hist.packed else 0,
+        self._stream())
+    self.launches += 1
+    self._check("batch_rts_ragged_segment")
+    return xs, Ps
+
 
 class _PackedGraph:
   """A captured graph of an engine with packed resident P: the graph reads and writes the full buffer, so before a

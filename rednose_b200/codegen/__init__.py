@@ -374,6 +374,14 @@ def gen_code(folder, name, f_sym, dt_sym, x_sym, obs_eqs, dim_x, dim_err, eskf_p
   brr = "const double *hx_pred, const double *hP_pred, const double *hx_filt, const double *hP_filt, const double *t, const int *len, double *xs, double *Ps, int T, long long B, const int *quat_idxs, int n_quat, int norm_quats, void *stream"
   hdr.append(f"int {name}_batch_rts_ragged({brr});")
   c.append(f'extern "C" int {name}_batch_rts_ragged({brr}) {{ return rnb::call_status([&] {{ rnb::batch_rts_ragged<{model}>(ctx_(), hx_pred, hP_pred, hx_filt, hP_filt, t, len, xs, Ps, T, B, quat_idxs, n_quat, norm_quats, stream); }}); }}\n')
+  # one SEGMENT of a ragged history: filter b's rows are its global rows k0[b] ..; with term[b] its row len[b] - 1 is the
+  # first row of its segment behind and the recursion starts from (x_term[b], P_term[b]).  packed selects the packed
+  # covariance layout (an argument, not a _packed name).  int result (see _hist_idx); refused above EDIM 32
+  brg = ("const double *hx_pred, const double *hP_pred, const double *hx_filt, const double *hP_filt, const double *t, const int *len, "
+         "const unsigned char *term, const long long *k0, const double *x_term, const double *P_term, double *xs, double *Ps, int T, "
+         "long long B, const int *quat_idxs, int n_quat, int norm_quats, int packed, void *stream")
+  hdr.append(f"int {name}_batch_rts_ragged_segment({brg});")
+  c.append(f'extern "C" int {name}_batch_rts_ragged_segment({brg}) {{ return rnb::call_status([&] {{ rnb::batch_rts_ragged_segment<{model}>(ctx_(), hx_pred, hP_pred, hx_filt, hP_filt, t, len, term, k0, x_term, P_term, xs, Ps, T, B, quat_idxs, n_quat, norm_quats, packed, stream); }}); }}\n')
   # the three smoothers over packed histories (REDNOSE_PACKED_HIST): hP_pred, hP_filt, Ps and P_term are
   # [.., <name>_packed_P_doubles()]; int results like the ragged ones, refused where the pair kernel does not record them
   for suffix, args, call in (("rts", br, f"batch_rts<{model}, true>(ctx_(), hx_pred, hP_pred, hx_filt, hP_filt, t, t_per_filter, xs, Ps, T, B, quat_idxs, n_quat, norm_quats, stream)"),

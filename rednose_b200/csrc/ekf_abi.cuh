@@ -399,6 +399,41 @@ inline void batch_rts_ragged(HostCtx<M>& ctx, const double* hx_pred, const doubl
   else launch_rts_auto<M, PH>(a, (cudaStream_t)stream);
 }
 
+// RTS over one SEGMENT of a ragged history: filter b smooths rows 0 .. len[b] - 1, the global rows k0[b] .. of its
+// stream; with term[b] != 0 row len[b] - 1 is the first row of the filter's segment behind (only its predicted state and
+// time are read) and the recursion starts from x_term[b] / P_term[b], that row's smoothed estimate.  packed: every
+// covariance slab, P_term included, is in the packed layout
+template <class M>
+inline void batch_rts_ragged_segment(HostCtx<M>& ctx, const double* hx_pred, const double* hP_pred, const double* hx_filt,
+                                     const double* hP_filt, const double* t, const int* len, const unsigned char* term,
+                                     const long long* k0, const double* x_term, const double* P_term, double* xs, double* Ps,
+                                     int T, long long B, const int* quat_idxs, int n_quat, int norm_quats, int packed,
+                                     void* stream) {
+  if (packed && !check_packed_hist<M, true>("batch_rts_ragged_segment")) return;
+  if constexpr (M::EDIM > 32) {
+    fprintf(stderr, "[rednose_b200] batch_rts_ragged_segment: ragged histories exist only up to EDIM 32 (EDIM = %d)\n", M::EDIM);
+    last_status() = (int)cudaErrorNotSupported;
+  } else {
+    if (B < 0 || (B > 0 && (!t || !len || !term || !k0 || !x_term || !P_term || T <= 0))) {
+      fprintf(stderr, "[rednose_b200] batch_rts_ragged_segment: B >= 0 and, for B > 0, per-filter times, lengths, terminal "
+                      "flags, first rows, terminal estimates and T >= 1 are required\n");
+      last_status() = (int)cudaErrorInvalidValue;
+      return;
+    }
+    if (!check_quat_idxs(quat_idxs, n_quat, M::DIM)) return;
+    RtsArgs<M::NG> a;
+    memset(&a, 0, sizeof(a));
+    a.hx_pred = hx_pred; a.hP_pred = hP_pred; a.hx_filt = hx_filt; a.hP_filt = hP_filt;
+    a.t = t; a.t_per_filter = 1; a.len = len; a.term = term; a.k0s = k0; a.x_term = x_term; a.P_term = P_term;
+    a.xs = xs; a.Ps = Ps; a.T = T; a.B = B; a.norm_quats = norm_quats;
+    a.n_quat = n_quat;
+    for (int i = 0; i < n_quat; ++i) a.quat_idx[i] = quat_idxs[i];
+    for (int i = 0; i < (M::NG > 0 ? M::NG : 1); ++i) a.gv[i] = ctx.gv.v[i];
+    if (!packed) launch_rts_ragged_segment<M, false>(a, (cudaStream_t)stream);
+    else if constexpr (pair_may_serve<M>()) launch_rts_ragged_segment<M, true>(a, (cudaStream_t)stream);   // refused above otherwise
+  }
+}
+
 // ------------------------------------------------------ covariance layout conversion ---
 // Entry e of the compact full-layout buffer `full` [n, EDIM, EDIM] <-> filter idx[e] (e without a list) of the packed
 // batch `packed` [*, packed_doubles(EDIM)].  Packing reads only the lower triangle; unpacking writes its exact mirror.

@@ -58,6 +58,20 @@ struct MainHistOf<M, decltype(void(M::MAIN_HIST))> { static constexpr bool value
 template <class M>
 constexpr bool main_hist() { return MainHistOf<M>::value; }
 
+// A filter model (EDIM <= 32) whose ragged history holds one SEGMENT of each filter's rows (RtsArgs::term / k0s): the
+// ragged smoothers are instantiated with RaggedSeg<M> (or RaggedSeg<PackedHist<M>>) in place of M, like PackedHist, so
+// the whole-history instantiations keep their symbols and machine code.
+template <class M>
+struct RaggedSeg : M {
+  static constexpr bool RAGGED_SEG = true;
+};
+template <class M, class = void>
+struct RaggedSegOf { static constexpr bool value = false; };
+template <class M>
+struct RaggedSegOf<M, decltype(void(M::RAGGED_SEG))> { static constexpr bool value = M::RAGGED_SEG; };
+template <class M>
+constexpr bool ragged_seg() { return RaggedSegOf<M>::value; }
+
 // One argument block per launch, passed by value (lives in the kernel parameter
 // constant bank: every field is warp-uniform).  NG = number of global_vars.
 template <int NG>

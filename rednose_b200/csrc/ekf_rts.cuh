@@ -63,11 +63,18 @@ struct RtsArgs {
   long long k0;
   double gv[NG > 0 ? NG : 1];
   // ragged histories: filter b smooths rows 0 .. len[b] - 1 only (with t [T, B]) and leaves its rows >= len[b] of xs / Ps
-  // untouched; nullptr = every filter has T rows.  Not combined with segment continuation.
+  // untouched; nullptr = every filter has T rows.  Combined with segment continuation only through RaggedSeg (below).
   const int* len;
   // M = MainHist<model> (EDIM > 32): hP_pred is [T, B, MEDIM, MEDIM], the main block of each P_{k|k-1}, and the recursion
   // starts (without x_term / P_term) from this [B, EDIM, EDIM] full P_{T-1|T-2}
   const double* hP_pred_last;
+  // M = RaggedSeg<model> (a ragged history holding one segment of each filter's rows, with len): term[b] != 0 makes row
+  // len[b] - 1 of filter b the first row of its segment behind, which contributes only its predicted state and time, and
+  // the recursion of filter b starts from x_term[b] / P_term[b], the smoothed estimate of that row (row len[b] - 1 of
+  // xs / Ps is then not written); term[b] == 0 smooths filter b as a whole ragged history does.  k0s[b] is the global
+  // row index of filter b's row 0 (normalisation: every output but global row 0).  Read only by those instantiations.
+  const unsigned char* term;
+  const long long* k0s;
 };
 
 // rows filter b smooths: T, or len[b] clamped to [0, T] for a ragged history
@@ -120,6 +127,7 @@ __global__ void __launch_bounds__(RTS_WARPS * 32, RTS_MIN_CTAS) ekf_rts_warp(con
   static_assert(N <= 32, "warp-per-filter RTS needs MEDIM <= 32");
   static_assert(E <= 32 || (!PH && !RAGGED), "above EDIM 32 only whole and segment histories in the full layout");
   static_assert(!PH || E % 2 == 0, "the packed layout needs an even EDIM");
+  static_assert(!ragged_seg<M>() || (RAGGED && E <= 32), "ragged segments are ragged histories, EDIM <= 32");
   static_assert(!MH || E > 32, "main-block prediction histories exist only above EDIM 32");
   constexpr int PS = PH ? packed_doubles(E) : E * E;   // doubles of one filter's covariance in the slabs
   constexpr int PPS = MH ? N * N : PS, PLD = MH ? N : E;   // the same, and the row stride, in the hP_pred slab
@@ -149,7 +157,7 @@ __global__ void __launch_bounds__(RTS_WARPS * 32, RTS_MIN_CTAS) ekf_rts_warp(con
   double pn[N];  // column `lane` of the carried smoothed covariance (main block)
   {
     const long long k = T - 1;
-    const bool seg = a.x_term != nullptr;
+    const bool seg = ragged_seg<M>() ? a.term[b] != 0 : a.x_term != nullptr;
     if constexpr (PH) {
       const double* Pg = seg ? a.P_term + b * (long long)PS : a.hP_pred + k * BP + b * (long long)PS;
       double* Po = a.Ps + k * BP + b * (long long)PS;
@@ -176,7 +184,7 @@ __global__ void __launch_bounds__(RTS_WARPS * 32, RTS_MIN_CTAS) ekf_rts_warp(con
     for (int i = lane; i < D; i += 32) s.xn[i] = seg ? a.x_term[b * D + i] : a.hx_pred[k * BX + b * D + i];
     __syncwarp();
     if (!seg) {
-      if (a.norm_quats && a.k0 + T - 1 >= 1) normalize_xn();   // every output but global index 0, as in the loop
+      if (a.norm_quats && (ragged_seg<M>() ? a.k0s[b] : a.k0) + T - 1 >= 1) normalize_xn();   // every output but global index 0, as in the loop
       for (int i = lane; i < D; i += 32) a.xs[k * BX + b * D + i] = s.xn[i];
     }
   }
@@ -279,7 +287,7 @@ __global__ void __launch_bounds__(RTS_WARPS * 32, RTS_MIN_CTAS) ekf_rts_warp(con
     __syncwarp();
     for (int i = lane; i < D; i += 32) s.xn[i] = (i < D1) ? s.xt[i] : s.xf[i];
     __syncwarp();
-    if (a.norm_quats && k + a.k0 >= 1) normalize_xn();
+    if (a.norm_quats && k + (ragged_seg<M>() ? a.k0s[b] : a.k0) >= 1) normalize_xn();
     for (int i = lane; i < D; i += 32) a.xs[k * BX + b * D + i] = s.xn[i];
 
     // ---- covariance: P_{k|N} = P_{k|k} + X^T (dP X) ----

@@ -14,6 +14,7 @@
 // results agree with the scalar kernel to rounding (different summation order).  Above EDIM 32 (an MSCKF) only the main
 // block of the slabs is read and written, as in ekf_rts_warp.
 #pragma once
+#include <type_traits>
 #include "ekf_rts.cuh"
 
 namespace rnb {
@@ -52,6 +53,7 @@ __global__ void __launch_bounds__(RTS_WARPS * 32, RTS_MIN_CTAS) ekf_rts_warp_mma
   static_assert(E % 2 == 0 && N <= 32, "fragment I/O needs an even EDIM and MEDIM <= 32");
   static_assert(E <= 32 || (!PH && !RAGGED), "above EDIM 32 only whole and segment histories in the full layout");
   static_assert(!MH || E > 32, "main-block prediction histories exist only above EDIM 32");
+  static_assert(!ragged_seg<M>() || (RAGGED && E <= 32), "ragged segments are ragged histories, EDIM <= 32");
   constexpr int PS = PH ? packed_doubles(E) : E * E;   // doubles of one filter's covariance in the slabs
   constexpr int PPS = MH ? N * N : PS, PLD = MH ? N : E;   // the same, and the row stride, in the hP_pred slab
   // dynamic: from a main block of 25 (NP = 32) the RTS_WARPS scratch blocks pass the 48 KB static limit
@@ -96,7 +98,7 @@ __global__ void __launch_bounds__(RTS_WARPS * 32, RTS_MIN_CTAS) ekf_rts_warp_mma
   double pn[NT * NT * 2];
   {
     const long long k = T - 1;
-    const bool seg = a.x_term != nullptr;   // segment continuation: start from the smoothed estimate handed in
+    const bool seg = ragged_seg<M>() ? a.term[b] != 0 : a.x_term != nullptr;   // segment continuation: start from the smoothed estimate handed in
     const double* Pg = seg ? a.P_term + b * (long long)PS
                            : (MH ? a.hP_pred_last + b * (long long)PS : a.hP_pred + k * BP + b * (long long)PS);
     double* Po = a.Ps + k * BP + b * (long long)PS;
@@ -113,7 +115,7 @@ __global__ void __launch_bounds__(RTS_WARPS * 32, RTS_MIN_CTAS) ekf_rts_warp_mma
     for (int i = lane; i < D; i += 32) s.xn[i] = seg ? a.x_term[b * D + i] : a.hx_pred[k * BX + b * D + i];
     __syncwarp();
     if (!seg) {
-      if (a.norm_quats && a.k0 + T - 1 >= 1) normalize_xn();   // every output but global index 0, as in the loop
+      if (a.norm_quats && (ragged_seg<M>() ? a.k0s[b] : a.k0) + T - 1 >= 1) normalize_xn();   // every output but global index 0, as in the loop
       for (int i = lane; i < D; i += 32) a.xs[k * BX + b * D + i] = s.xn[i];
     }
   }
@@ -259,7 +261,7 @@ __global__ void __launch_bounds__(RTS_WARPS * 32, RTS_MIN_CTAS) ekf_rts_warp_mma
     __syncwarp();
     for (int i = lane; i < D; i += 32) s.xn[i] = (i < D1) ? s.xt[i] : s.xf[i];
     __syncwarp();
-    if (a.norm_quats && k + a.k0 >= 1) normalize_xn();
+    if (a.norm_quats && k + (ragged_seg<M>() ? a.k0s[b] : a.k0) >= 1) normalize_xn();
     for (int i = lane; i < D; i += 32) a.xs[k * BX + b * D + i] = s.xn[i];
 
     // ---- X into shared memory, row-major, zero padded (lane j writes column j) ----
@@ -375,6 +377,27 @@ inline void launch_rts_auto(const RtsArgs<M::NG>& a, cudaStream_t st) {
     last_status() = (int)cudaErrorNotSupported;
   } else {
     launch_rts<M, PH>(a, st);
+  }
+}
+
+// one segment of a ragged history (a.len, a.term, a.k0s, a.x_term / a.P_term; EDIM <= 32): the RaggedSeg instantiations
+// of the kernel launch_rts_auto picks for M.  PH: the covariance slabs are packed (callers check that the pair kernel
+// serves M)
+template <class M, bool PH>
+inline void launch_rts_ragged_segment(const RtsArgs<M::NG>& a, cudaStream_t st) {
+  static_assert(M::EDIM <= 32, "ragged histories exist only up to EDIM 32");
+  if (a.B <= 0 || a.T <= 0) return;
+  using MS = RaggedSeg<std::conditional_t<PH, PackedHist<M>, M>>;
+  const unsigned grid = (unsigned)((a.B + RTS_WARPS - 1) / RTS_WARPS);
+  if constexpr (M::EDIM % 2 == 0 && M::MEDIM >= 8 && M::MEDIM <= 32) {
+    constexpr size_t smem = sizeof(RtsMmaScratch<MS>) * RTS_WARPS;
+    auto kern = ekf_rts_warp_mma<MS, true>;
+    if (first_launch_of((const void*)kern)) cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    kern<<<grid, RTS_WARPS * 32, smem, st>>>(a);
+    check(cudaGetLastError(), "ekf_rts_mma launch");
+  } else {
+    ekf_rts_warp<MS, true><<<grid, RTS_WARPS * 32, 0, st>>>(a);
+    check(cudaGetLastError(), "ekf_rts launch");
   }
 }
 

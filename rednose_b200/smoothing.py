@@ -243,3 +243,147 @@ class CheckpointedSmoother:
     self.stats = {"tiles": tiles, "tile_filters": n_tile, "segments": nseg, "segment_steps": S, "forward_ms": fwd_ms, "reforward_with_history_ms": refwd_ms,
                   "backward_ms": bwd_ms, "bytes_per_filter": self.bytes_per_filter(T)}
     return tiles
+
+
+def ragged_history_bytes_per_filter(dim_x, dim_err, T, packed_doubles=0):
+  """Bytes of one filter's share of a RaggedHistory of T rows (BatchedEKF.new_ragged_history(T)): the four slabs, the
+  per-filter times and the row count."""
+  return history_bytes_per_filter(dim_x, dim_err, T, packed_doubles=packed_doubles) + 8 * T + 4
+
+
+class RaggedCheckpointedSmoother(CheckpointedSmoother):
+  """Forward filter + RTS smoother over RAGGED streams (filters on their own clocks, RaggedScheduler) too long for one
+  RaggedHistory, in equal tiles of filters planned from the HBM budget like CheckpointedSmoother.
+
+  A whole RaggedHistory is padded to the longest stream (T * B * 8 120 bytes for live, 4 600 packed).  Here the stream is
+  cut into segments of `segment` TICKS.  Pass 1 runs RaggedScheduler without a history and, before the first tick of
+  every segment, checkpoints each filter's x, P, clock and rows so far (it steps through the same recording kernels as
+  the re-forward, into a history of one row); it also counts each filter's rows per segment,
+  whose maximum (+ 1) sizes the one segment history, so no tick waits for the host.  The backward sweep then visits the
+  segments last to first: it restores the checkpoint, replays the segment's ticks through RaggedScheduler(history=...),
+  appends to each filter the first row of its next segment that has rows (its predicted state and time; the carried
+  row), and smooths every filter over its own rows from the smoothed estimate of that carried row
+  (BatchedEKF.rts_smooth_ragged_segment).  A filter's row 0 then becomes its carried row and terminal estimate for the
+  segments in front; a filter without rows in a segment keeps the one it carries.  Each filter's rows come out bit for
+  bit as one whole RaggedHistory + rts_smooth would give them (the kernels are deterministic).  Memory per filter is one
+  checkpoint per segment plus a segment history; the price is a second forward pass.
+
+  Observations that arrive late are dropped by RaggedScheduler, as in a single pass.  Streams with late observations are
+  for RewindingScheduler, which records the rows RaggedScheduler would record for the same observations in time-stamp
+  order (DESIGN.md section 4.7): for offline smoothing, sort such a stream by time stamp first and smooth it here.
+  Feature-track kinds that augment the state are not driven (step_indexed does not augment).
+
+  packed_history=True: the segment history, the carried rows and terminal estimates and the covariances the sink receives
+  are packed ([..., packed doubles]; unpack_P gives them full); the checkpoints stay full."""
+
+  def __init__(self, folder, name, Q, dim_x, dim_err, quaternion_idxs=(), device="cuda", hbm_budget_bytes=60 << 30, segment=64, tile=None,
+               packed_history=False):
+    super().__init__(folder, name, Q, dim_x, dim_err, quaternion_idxs=quaternion_idxs, device=device,
+                     hbm_budget_bytes=hbm_budget_bytes, segment=segment, tile=tile, packed_history=packed_history)
+
+  def bytes_per_filter(self, n_ticks):
+    """Per filter: a checkpoint per segment (x, P, clock, rows so far, rows in the segment), a segment history of at most
+    `segment` + 1 rows (a filter records at most one row per tick, + the carried row) and pass 1's history of one row,
+    the carried row and terminal estimate, and the resident state with its scheduler clock."""
+    nseg = (n_ticks + self.segment - 1) // self.segment
+    state = 8 * (self.dim_err**2 + self.dim_x)
+    cov = self.packed_doubles or self.dim_err**2
+    hist = sum(ragged_history_bytes_per_filter(self.dim_x, self.dim_err, T, self.packed_doubles) for T in (self.segment + 1, 1))
+    return nseg * (state + 8 + 8 + 4) + hist + 8 * (2 * self.dim_x + 2 * cov + 1) + 3 * state + 2 * 8
+
+  def run(self, x0, P0, n_ticks, tick_fn, sink, norm_quats=False):
+    """x0 [B, DIM], P0 [B, EDIM, EDIM] (host or device).  tick_fn(j, lo, hi) returns tick j of filters lo..hi as the
+    arguments of RaggedScheduler.tick, with filter ids local to the tile: (filter_ids, t, kinds, z_by_kind, R_by_kind) or
+    those and ea_by_kind.  It must return the same tick every time it is asked for j (each tick is filtered twice).
+
+    sink(lo, hi, k0 [n], n_rows [n], xs [rows, n, DIM], Ps [rows, n, EDIM, EDIM]) receives, segment by segment (last to
+    first), the smoothed rows of filters lo..hi: rows 0 .. n_rows[b] - 1 of filter b are its global rows k0[b] .. (its
+    k-th applied observation is its global row k).  Device views, valid during the call only; Ps [rows, n, packed doubles]
+    with packed_history.  Returns the number of tiles."""
+    from rednose_b200.scheduler import RaggedScheduler
+    B, S = x0.shape[0], self.segment
+    n_tile, _ = self.plan(B, n_ticks)
+    nseg = (n_ticks + S - 1) // S
+    dev, f64 = self.device, dict(dtype=torch.float64, device=self.device)
+    ev = [torch.cuda.Event(enable_timing=True) for _ in range(2)]
+    fwd_ms = refwd_ms = bwd_ms = 0.0
+    tiles, max_rows = 0, 0
+    for lo in range(0, B, n_tile):
+      hi = min(lo + n_tile, B)
+      n = hi - lo
+      if self._engine is None or self._engine.B != n:
+        self._engine = self._hist = self._ck = None     # release the previous tile's buffers before allocating
+        self._engine = BatchedEKF(self.folder, self.name, self.Q, x0[lo:hi], P0[lo:hi], device=dev, quaternion_idxs=self.quat)
+      else:
+        self._engine.init_state(x0[lo:hi], P0[lo:hi], None)
+      eng = self._engine
+      if self._ck is None or self._ck[0].shape[0] != nseg:
+        self._ck = None
+        self._ck = (torch.empty(nseg, n, self.dim_x, **f64), torch.empty(nseg, n, self.dim_err, self.dim_err, **f64),
+                    torch.empty(nseg, n, **f64), torch.empty(nseg, n, dtype=torch.int64, device=dev),
+                    torch.empty(nseg, n, dtype=torch.int32, device=dev))
+      ck_x, ck_P, ck_t, ck_k0, rows = self._ck
+      rows.zero_()
+      # ---- pass 1: forward; checkpoint before the first tick of every segment, count rows per segment.  It steps through
+      # the recording gather kernels like the re-forward, so that the checkpoints are bit for bit the states the re-forward
+      # reaches (the gather kernels with and without history rows are separate instantiations, which need not round
+      # alike); into a history of one row, which every later step finds used up and does not record into ----
+      sched = RaggedScheduler(eng, history=eng.new_ragged_history(1, packed=bool(self.packed_doubles)))
+      done = torch.zeros(n, dtype=torch.int64, device=dev)
+      ev[0].record()
+      for j in range(nseg):
+        ck_x[j].copy_(eng.x); ck_P[j].copy_(eng.P); ck_t[j].copy_(sched.t_filter); ck_k0[j].copy_(done)
+        for tick in range(j * S, min((j + 1) * S, n_ticks)):
+          for ids, _ in sched.tick(*tick_fn(tick, lo, hi)).values():
+            rows[j].index_add_(0, ids, torch.ones_like(ids, dtype=torch.int32))
+        done += rows[j]
+      ev[1].record(); ev[1].synchronize(); fwd_ms += ev[0].elapsed_time(ev[1])
+      T = int(rows.max()) + 1                           # the longest segment of any filter + its carried row
+      max_rows = max(max_rows, T - 1)
+      if self._hist is None or self._hist.T != T:
+        self._hist = None
+        self._hist = eng.new_ragged_history(T, packed=bool(self.packed_doubles))
+      hist = self._hist
+      cov = hist.P_filt.shape[2:]
+      # the carried row (x_pred, P_pred, t) of every filter and its smoothed estimate (the terminal)
+      cx, cP, ct = torch.empty(n, self.dim_x, **f64), torch.empty(n, *cov, **f64), torch.empty(n, **f64)
+      tx, tP = torch.empty(n, self.dim_x, **f64), torch.empty(n, *cov, **f64)
+      carry = torch.zeros(n, dtype=torch.bool, device=dev)
+      ar = torch.arange(n, device=dev)
+      sched = RaggedScheduler(eng, history=hist)
+      # ---- backward sweep: segments last to first, each re-filtered with history from its checkpoint, then smoothed ----
+      for j in range(nseg - 1, -1, -1):
+        eng.x.copy_(ck_x[j]); eng.P.copy_(ck_P[j]); sched.t_filter.copy_(ck_t[j])
+        hist.n.zero_(); hist.overflow.zero_()
+        ev[0].record()
+        for tick in range(j * S, min((j + 1) * S, n_ticks)):
+          sched.tick(*tick_fn(tick, lo, hi))
+        ev[1].record(); ev[1].synchronize(); refwd_ms += ev[0].elapsed_time(ev[1])
+        lost = hist.overflowed()
+        if lost:
+          raise RuntimeError(f"segment {j} (ticks {j * S} .. {min((j + 1) * S, n_ticks) - 1}) overflowed its history of {T} "
+                             f"rows by {lost} step(s): the stream differs from pass 1; use a shorter segment")
+        nr = hist.n.clone()
+        term = carry & (nr > 0)
+        r = nr.clamp(max=T - 1).to(torch.int64)         # row n[b]: the carried row of the filters with a terminal
+        hist.x_pred[r, ar] = torch.where(term[:, None], cx, hist.x_pred[r, ar])
+        hist.P_pred[r, ar] = torch.where(term.view(-1, *[1] * len(cov)), cP, hist.P_pred[r, ar])
+        hist.t[r, ar] = torch.where(term, ct, hist.t[r, ar])
+        hist.n += term.to(torch.int32)
+        ev[0].record()
+        xs, Ps = eng.rts_smooth_ragged_segment(hist, term, ck_k0[j], (tx, tP), norm_quats=norm_quats,
+                                               quaternion_idxs=self.quat or (3,), in_place=True)
+        ev[1].record(); ev[1].synchronize(); bwd_ms += ev[0].elapsed_time(ev[1])
+        has = nr > 0                                    # row 0 hands over to the segments in front
+        cx.copy_(torch.where(has[:, None], hist.x_pred[0], cx))
+        cP.copy_(torch.where(has.view(-1, *[1] * len(cov)), hist.P_pred[0], cP))
+        ct.copy_(torch.where(has, hist.t[0], ct))
+        tx.copy_(torch.where(has[:, None], xs[0], tx))
+        tP.copy_(torch.where(has.view(-1, *[1] * len(cov)), Ps[0], tP))
+        carry |= has
+        sink(lo, hi, ck_k0[j], nr, xs, Ps)
+      tiles += 1
+    self.stats = {"tiles": tiles, "tile_filters": n_tile, "segments": nseg, "segment_ticks": S, "segment_rows": max_rows,
+                  "forward_ms": fwd_ms, "reforward_with_history_ms": refwd_ms, "backward_ms": bwd_ms,
+                  "bytes_per_filter": self.bytes_per_filter(n_ticks)}
+    return tiles
