@@ -32,6 +32,10 @@
  *     int <name>_batch_restore_hist(...)   filter idx[e] of the resident x / P <- row hist_row[e] (negative: skipped) of
  *         the x_filt / P_filt slabs, the estimate that row recorded (a rewind to it).  REDNOSE_PACKED_HIST gives the slabs'
  *         layout, REDNOSE_PACKED_P the resident one, any pair of them.  EDIM <= 32 only (cudaErrorNotSupported otherwise)
+ *     int <name>_batch_augment_idx(double *x, double *P, const int *idx, long long n, int flags, void *stream)   MSCKF
+ *         libraries only: the clone-window shift of <name>_batch_augment (ekf_sym.py:365-391) for the n filters idx[e],
+ *         which must be distinct; the others are untouched.  Full covariance layout: REDNOSE_PACKED_P / _HIST are refused
+ *         (cudaErrorNotSupported), n < 0 or, for n > 0, a null pointer is cudaErrorInvalidValue; n = 0 launches nothing
  *   batched, HOST pointers (copies inside): <name>_host_step_<kind>(...)
  *   packed covariance layout (int results, so the reference's `void ` prototype set is unchanged):
  *     int <name>_packed_P_doubles(void)   doubles per filter of the packed layout, 0 where it is not used
@@ -89,6 +93,8 @@ typedef int (*rednose_batch_rts_ragged_fn)(const double *hx_pred, const double *
 typedef int (*rednose_batch_rts_ragged_segment_fn)(const double *hx_pred, const double *hP_pred, const double *hx_filt, const double *hP_filt, const double *t, const int *len, const unsigned char *term, const long long *k0, const double *x_term, const double *P_term, double *xs, double *Ps, int T, long long B, const int *quat_idxs, int n_quat, int norm_quats, int packed, void *stream);
 /* ragged histories: filter idx[e] of the resident x / P <- slab element hist_row[e] * hist_B + idx[e] of hx_filt / hP_filt */
 typedef int (*rednose_batch_restore_hist_fn)(const double *hx_filt, const double *hP_filt, const int *idx, const int *hist_row, long long n, long long hist_B, double *x, double *P, int flags, void *stream);
+/* MSCKF libraries: the clone-window shift of the n filters idx[e] (distinct) of the full-layout x / P */
+typedef int (*rednose_batch_augment_idx_fn)(double *x, double *P, const int *idx, long long n, int flags, void *stream);
 
 /* Plugin descriptor: replaces `struct EKF` (ekf.h:16-33).  Arrays have n_kinds entries,
  * parallel to `kinds`. */

@@ -100,6 +100,8 @@ class BatchedEKF:
     if np.count_nonzero(Qh - np.diag(np.diagonal(Qh))) == 0:
       self.flags |= Q_IS_DIAGONAL  # lets the kernels skip the dense dt*Q read
     self.kinds = sorted(int(s[len(name) + 12:]) for s in dir(self._lib) if s.startswith(f"{name}_batch_step_") and not s.endswith("_idx"))
+    # feature-track kinds (those with an He leaf): the CTA-per-filter kernel runs them at any EDIM
+    self._feature_kinds = {k for k in self.kinds if hasattr(self._lib, f"{name}_He_{k}")}
     self._zdim = {}
     self.launches = 0  # kernels launched through this object (bench.py reports it)
     for g, v in (global_vars or {}).items():
@@ -260,13 +262,49 @@ class BatchedEKF:
     self._check(f"batch_update_{kind}")
     return z
 
-  def step_indexed(self, kind, idx, dt, z, R, ea=None, hist=None, t=None):
+  def step_indexed(self, kind, idx, dt, z, R, ea=None, hist=None, t=None, augment=False):
     """Fused predict + update of `kind` for the filters listed in `idx` only ([n] int32, device): entry e uses
     z[e], R[e] (or one shared R), dt[e] and works on filter idx[e].  Filters not listed are untouched.  This is the
     building block of the ragged scheduler (per-tick kind buckets).
 
     With a RaggedHistory `hist`, entry e also records its step at filter idx[e]'s next row, with time t[e] (scalar
-    or [n]); a filter whose T rows are used up still steps and counts an overflow."""
+    or [n]); a filter whose T rows are used up still steps and counts an overflow.
+
+    augment (MSCKF): True, or an [n] bool mask aligned with `idx`: the flagged filters shift their clone window after
+    their update, as predict_and_update_batch(..., augment=True) (ekf_sym.py:527-528); a recorded row keeps the estimate
+    before the shift.  Kinds the CTA-per-filter kernel runs (EDIM > 32, or a feature-track kind) shift inside their own
+    gather launch (the fused shift); the others step in one launch and shift the flagged filters in a second one.  The
+    innovations keep the order of `idx`."""
+    if augment is None or augment is False:
+      return self._step_indexed(kind, idx, dt, z, R, ea, hist, t)
+    idx = idx.to(device=self.device, dtype=torch.int32).contiguous()
+    n = int(idx.shape[0])
+    mask = torch.as_tensor(augment, device=self.device).to(torch.bool).expand(n)
+    if not bool(mask.any()):
+      return self._step_indexed(kind, idx, dt, z, R, ea, hist, t)
+    if not (self.dim_err > 32 or kind in self._feature_kinds):
+      y = self._step_indexed(kind, idx, dt, z, R, ea, hist, t)
+      self.augment(idx[mask])
+      return y
+    # the fused shift: the flagged entries in a gather launch of their own with the AUGMENT flag
+    z = _as_device(z, self.device)
+    if z.ndim == 2:
+      z = z.unsqueeze(1)
+    R = _as_device(R, self.device)
+    ea = _as_device(ea, self.device) if ea is not None else None
+    if t is not None and torch.as_tensor(t).ndim == 1:
+      t = torch.as_tensor(t, dtype=torch.float64, device=self.device)
+    for sel, aug in (((~mask).nonzero(as_tuple=True)[0], 0), (mask.nonzero(as_tuple=True)[0], AUGMENT)):
+      if sel.numel() == 0:
+        continue
+      dt_s = dt.to(self.device)[sel] if isinstance(dt, torch.Tensor) else dt
+      t_s = t[sel] if isinstance(t, torch.Tensor) and t.ndim == 1 else t
+      y = self._step_indexed(kind, idx[sel], dt_s, z[sel], R if R.ndim == 2 else R[sel], None if ea is None else ea[sel],
+                             hist, t_s, extra_flags=aug)
+      z[sel] = y
+    return z
+
+  def _step_indexed(self, kind, idx, dt, z, R, ea=None, hist=None, t=None, extra_flags=0):
     idx = idx.to(device=self.device, dtype=torch.int32).contiguous()
     n = int(idx.shape[0])
     if n == 0:
@@ -275,7 +313,7 @@ class BatchedEKF:
     if z.ndim == 2:
       z = z.unsqueeze(1)
     R = _as_device(R, self.device)
-    flags = self.flags
+    flags = self.flags | extra_flags
     if R.ndim == 2:
       flags |= SHARED_R
     elif R.ndim == 3:
@@ -424,12 +462,24 @@ class BatchedEKF:
     d = self.maha_dist(kind, z, R, ea)
     return d <= float(chi2_ppf(maha_thresh, z.shape[-1] if hasattr(z, "shape") else len(z[0])))
 
-  def augment(self):
-    """MSCKF clone window shift for the whole batch (ekf_sym.py:365-391), one launch."""
+  def augment(self, ids=None):
+    """MSCKF clone window shift (ekf_sym.py:365-391), one launch: for the whole batch, or with `ids` ([m] int, distinct,
+    device or host) for those filters only.  The shift works on the full covariance: a packed resident P is unpacked
+    first (reading ``P``)."""
+    if ids is None:
+      with torch.cuda.device(self.device):
+        getattr(self._lib, f"{self.name}_batch_augment")(self._p(self.x), self._p(self.P), self.B, self._stream())
+      self.launches += 1
+      self._check("batch_augment")
+      return
+    ids = torch.as_tensor(ids, device=self.device).to(torch.int32).contiguous()
+    if ids.numel() == 0:
+      return
     with torch.cuda.device(self.device):
-      getattr(self._lib, f"{self.name}_batch_augment")(self._p(self.x), self._p(self.P), self.B, self._stream())   # EDIM > 32: never packed
+      getattr(self._lib, f"{self.name}_batch_augment_idx")(
+        self._p(self.x), self._p(self.P), self._ffi.cast("const int *", ids.data_ptr()), int(ids.shape[0]), 0, self._stream())
     self.launches += 1
-    self._check("batch_augment")
+    self._check("batch_augment_idx")
 
   # ------------------------------------------------------- history + smoothing ---
   def _history_doubles(self, packed):

@@ -409,6 +409,11 @@ def gen_code(folder, name, f_sym, dt_sym, x_sym, obs_eqs, dim_x, dim_err, eskf_p
     ba = "double *x, double *P, long long B, void *stream"
     hdr.append(f"void {name}_batch_augment({ba});")
     c.append(f'extern "C" void {name}_batch_augment({ba}) {{ rnb::launch_augment<{model}>(x, P, B, {int(dim_augment)}, {int(dim_augment_err)}, (cudaStream_t)stream); }}\n')
+    # the shift of the n filters idx[e] (distinct) only, for filters on their own clocks; full covariance layout (packed
+    # flags refused).  int result (see _hist_idx)
+    bai = "double *x, double *P, const int *idx, long long n, int flags, void *stream"
+    hdr.append(f"int {name}_batch_augment_idx({bai});")
+    c.append(f'extern "C" int {name}_batch_augment_idx({bai}) {{ return rnb::call_status([&] {{ rnb::launch_augment_idx<{model}>(x, P, idx, n, flags, {int(dim_augment)}, {int(dim_augment_err)}, (cudaStream_t)stream); }}); }}\n')
 
   # ---- descriptor + ekf_get (rednose/helpers/ekf.h:16-42) ----
   kl = [kd['kind'] for kd in kinds]

@@ -25,23 +25,27 @@ class RaggedScheduler:
     self.t_filter = torch.full((engine.B,), float("nan"), dtype=torch.float64, device=engine.device)
     self.dropped = 0
 
-  def tick(self, filter_ids, t, kinds, z_by_kind, R_by_kind, ea_by_kind=None):
+  def tick(self, filter_ids, t, kinds, z_by_kind, R_by_kind, ea_by_kind=None, augment=None):
     """One scheduling tick.
 
     filter_ids [n] int, t [n] float64 (or scalar), kinds [n] int: the observations of this tick, at most one per
     filter.  z_by_kind[k] is [n_k, m_k] in the order the entries of kind k appear in `filter_ids`;
-    R_by_kind[k] is [m_k, m_k] (shared) or [n_k, m_k, m_k].  Returns {kind: (filter_ids_k, innovations_k)}.
+    R_by_kind[k] is [m_k, m_k] (shared) or [n_k, m_k, m_k].  augment [n] bool (MSCKF), aligned with `filter_ids`: the
+    flagged filters shift their clone window after their observation (a camera frame: predict_and_update_batch(...,
+    augment=True)); a dropped observation neither steps nor shifts.  Returns {kind: (filter_ids_k, innovations_k)}.
     """
     dev = self.e.device
     fid = torch.as_tensor(filter_ids, device=dev).to(torch.int64)
     kinds = torch.as_tensor(kinds, device=dev)
     t = torch.as_tensor(t, dtype=torch.float64, device=dev).expand(fid.shape[0])
+    aug = None if augment is None else torch.as_tensor(augment, device=dev).to(torch.bool).expand(fid.shape[0])
     out = {}
     for k in sorted(z_by_kind):
       sel = (kinds == k).nonzero(as_tuple=True)[0]
       if sel.numel() == 0:
         continue
       ids, tk = fid[sel], t[sel]
+      ak = None if aug is None else aug[sel]
       tf = self.t_filter[ids]
       tf = torch.where(torch.isnan(tf), tk, tf)          # first observation initialises the clock (ekf_sym.py:502-503)
       dt = tk - tf
@@ -56,7 +60,11 @@ class RaggedScheduler:
           R = R[ok]
         if ea is not None:
           ea = ea[ok]
+        if ak is not None:
+          ak = ak[ok]
       rec = {} if self.history is None else dict(hist=self.history, t=tk)
+      if ak is not None and bool(ak.any()):               # only then: engines without clone windows take no augment=
+        rec["augment"] = ak
       y = self.e.step_indexed(k, ids.to(torch.int32), dt, z.clone(), R, ea, **rec)
       self.t_filter[ids] = tk
       out[k] = (ids, None if y is None else y[:, 0])
@@ -86,6 +94,16 @@ class RewindingScheduler(RaggedScheduler):
   filter's rows are what RaggedScheduler would have recorded had the same observations arrived in time order:
   engine.rts_smooth(history) smooths them.  A late observation whose checkpoint was stepped while the filter's rows were
   used up cannot be restored: it is ignored and counted in `.unrecorded` (the history has overflowed anyway).
+
+  MSCKF clone windows (tick(..., augment=)): each checkpoint keeps its observation's augment flag (`ring_aug`).  Without
+  a history the snapshot is the state after the shift, as the reference's checkpoint is (ekf_sym.py:525-529).  With one,
+  the checkpoint's row holds the estimate before the shift, so a rewind to a checkpoint whose observation shifted
+  restores from the row and shifts again (engine.augment(ids)); the shift is a permutation, so that is the reference's
+  checkpoint bit for bit.  Replays re-apply each observation's recorded shift.  This deliberately differs from the
+  reference, whose drivers drop the flag on replay (ekf_sym.py keeps (t, kind, z, R, extra_args) in its cache, ekf_sym.cc:110
+  replays with augment = false) and so leave the clone window one frame behind after a rewind over a camera frame.
+  Re-applying it keeps the rows recorded under rewinds equal to those RaggedScheduler records for the same observations
+  in time order.
   """
 
   def __init__(self, engine, zdims, depth=16, max_rewind_age=1.0, ea_dims=None, packed=False, history=None):
@@ -124,6 +142,8 @@ class RewindingScheduler(RaggedScheduler):
       else:
         self.ring_P = torch.zeros(B, self.N, E, E, **f64)
     self.ring_kind = torch.zeros(B, self.N, dtype=torch.int64, device=dev)
+    self.ring_aug = torch.zeros(B, self.N, dtype=torch.bool, device=dev)     # the observation shifted the clone window
+    self._augmenting = False                       # a tick has passed augment=: rewinds and replays look at ring_aug
     self.ring_z = torch.zeros(B, self.N, zmax, **f64)
     self.ring_R = torch.zeros(B, self.N, zmax, zmax, **f64)
     self.ring_ea = torch.zeros(B, self.N, eamax, **f64) if eamax else None
@@ -145,9 +165,9 @@ class RewindingScheduler(RaggedScheduler):
     else:
       self.e.P[ids] = P
 
-  def _push(self, ids, t, kind, z, R, ea, rows):
+  def _push(self, ids, t, kind, z, R, ea, rows, aug):
     """Checkpoint the CURRENT state of filters `ids` together with the observation just applied (ekf_sym.py:437-450);
-    with a history the state is the one recorded at `rows`."""
+    with a history the state is the one recorded at `rows` (before the shift of the entries flagged in `aug`)."""
     full = self.cnt[ids] == self.N
     pos = torch.where(full, self.head[ids], (self.head[ids] + self.cnt[ids]) % self.N)
     m = z.shape[-1]
@@ -159,6 +179,7 @@ class RewindingScheduler(RaggedScheduler):
       P = self._get_P(ids)
       self.ring_P[ids, pos] = P[:, self._tri_r, self._tri_c] if self.packed else P
     self.ring_kind[ids, pos] = kind
+    self.ring_aug[ids, pos] = False if aug is None else aug
     self.ring_z[ids, pos, :m] = z
     self.ring_R[ids, pos, :m, :m] = R
     if ea is not None and self.ring_ea is not None:
@@ -166,8 +187,9 @@ class RewindingScheduler(RaggedScheduler):
     self.head[ids] = torch.where(full, (self.head[ids] + 1) % self.N, self.head[ids])
     self.cnt[ids] = torch.where(full, self.cnt[ids], self.cnt[ids] + 1)
 
-  def _apply(self, ids, t, kinds, z, R, ea, want_y):
-    """Predict to t + update + checkpoint for entries (ids, t, kinds) with padded z / R / ea rows: one launch per kind."""
+  def _apply(self, ids, t, kinds, z, R, ea, aug, want_y):
+    """Predict to t + update (+ clone-window shift where `aug`, [n] bool or None) + checkpoint for entries (ids, t, kinds)
+    with padded z / R / ea rows: one launch per kind (and kernel)."""
     out = {}
     for k in torch.unique(kinds).tolist():
       sel = (kinds == k).nonzero(as_tuple=True)[0]
@@ -182,22 +204,28 @@ class RewindingScheduler(RaggedScheduler):
       if self.history is not None:                         # the row reserve() hands out; it saturates n, so read it first
         n = self.history.n[idk]
         rows, rec = torch.where(n < self.history.T, n, -1), dict(hist=self.history, t=tk)
+      ak = None if aug is None else aug[sel]
+      if ak is not None and bool(ak.any()):                # only then: engines without clone windows take no augment=
+        rec["augment"] = ak
       y = self.e.step_indexed(int(k), idk.to(torch.int32), (tk - tf).contiguous(), zk.clone(), Rk, eak, **rec)
       self.t_filter[idk] = tk
-      self._push(idk, tk, int(k), zk, Rk, eak, rows)
+      self._push(idk, tk, int(k), zk, Rk, eak, rows, ak)
       if want_y:
         out[int(k)] = (idk, None if y is None else y[:, 0])
     return out
 
   # -- one tick ---------------------------------------------------------------------------------------------------------
-  def tick(self, filter_ids, t, kinds, z_by_kind, R_by_kind, ea_by_kind=None):
+  def tick(self, filter_ids, t, kinds, z_by_kind, R_by_kind, ea_by_kind=None, augment=None):
     """Same arguments and return value as RaggedScheduler.tick; late observations rewind instead of being dropped
-    (those that the reference would ignore are counted in `.dropped` and absent from the result)."""
+    (those that the reference would ignore are counted in `.dropped` and absent from the result).  A late observation
+    flagged in `augment` shifts when it is applied, and every observation replayed after it shifts again if it did."""
     dev, N = self.e.device, self.N
     fid = torch.as_tensor(filter_ids, device=dev).to(torch.int64)
     kinds = torch.as_tensor(kinds, device=dev).to(torch.int64)
     n = int(fid.shape[0])
     t = torch.as_tensor(t, dtype=torch.float64, device=dev).expand(n).contiguous()
+    aug = None if augment is None else torch.as_tensor(augment, device=dev).to(torch.bool).expand(n).contiguous()
+    self._augmenting |= aug is not None
     zmax = self.ring_z.shape[-1]
     z = torch.zeros(n, zmax, dtype=torch.float64, device=dev)
     R = torch.zeros(n, zmax, zmax, dtype=torch.float64, device=dev)
@@ -245,6 +273,9 @@ class RewindingScheduler(RaggedScheduler):
           if self.history is not None:
             self.e.restore_from_history(self.history, lf, row)           # ekf_sym.py:425-427, from the recorded row
             self.history.rewind(lf, row)
+            shifted = self.ring_aug[lf, src] if self._augmenting else None   # the row holds the estimate before the shift
+            if shifted is not None and bool(shifted.any()):
+              self.e.augment(lf[shifted])
           else:
             self.e.x[lf] = self.ring_x[lf, src]                          # ekf_sym.py:425-427
             if self.packed:
@@ -259,18 +290,19 @@ class RewindingScheduler(RaggedScheduler):
           pp = phys.gather(1, lp)
           replay = dict(f=lf, n=n_rep, t=self.ring_t[lf[:, None], pp], kind=self.ring_kind[lf[:, None], pp],
                         z=self.ring_z[lf[:, None], pp], R=self.ring_R[lf[:, None], pp],
-                        ea=None if self.ring_ea is None else self.ring_ea[lf[:, None], pp])
+                        ea=None if self.ring_ea is None else self.ring_ea[lf[:, None], pp], aug=self.ring_aug[lf[:, None], pp] if self._augmenting else None)
           self.cnt[lf] = idx                                             # throw away the old future (ekf_sym.py:432-435)
           self.rewinds += int(lf.shape[0])
 
     out = {}
     if bool(keep.any()):
       ks = keep.nonzero(as_tuple=True)[0]
-      out = self._apply(fid[ks], t[ks], kinds[ks], z[ks], R[ks], None if ea is None else ea[ks], True)
+      out = self._apply(fid[ks], t[ks], kinds[ks], z[ks], R[ks], None if ea is None else ea[ks], None if aug is None else aug[ks], True)
     if replay is not None:                                               # fast-forward (ekf_sym.py:479-480)
       for r in range(int(replay["n"].max())):
         sel = (replay["n"] > r).nonzero(as_tuple=True)[0]
         self._apply(replay["f"][sel], replay["t"][sel, r].contiguous(), replay["kind"][sel, r], replay["z"][sel, r],
-                    replay["R"][sel, r], None if replay["ea"] is None else replay["ea"][sel, r], False)
+                    replay["R"][sel, r], None if replay["ea"] is None else replay["ea"][sel, r],
+                    None if replay["aug"] is None else replay["aug"][sel, r], False)
         self.replayed += int(sel.shape[0])
     return out

@@ -271,7 +271,9 @@ class RaggedCheckpointedSmoother(CheckpointedSmoother):
   Observations that arrive late are dropped by RaggedScheduler, as in a single pass.  Streams with late observations are
   for RewindingScheduler, which records the rows RaggedScheduler would record for the same observations in time-stamp
   order (DESIGN.md section 4.7): for offline smoothing, sort such a stream by time stamp first and smooth it here.
-  Feature-track kinds that augment the state are not driven (step_indexed does not augment).
+  MSCKF streams whose camera frames shift the clone window pass the ticks' augment flags (RaggedScheduler.tick's
+  `augment`); pass 1 and the re-forward both apply them.  Above EDIM 32 the smoothing step is refused
+  (rts_smooth_ragged_segment), so such filters are not smoothed here.
 
   packed_history=True: the segment history, the carried rows and terminal estimates and the covariances the sink receives
   are packed ([..., packed doubles]; unpack_P gives them full); the checkpoints stay full."""
@@ -293,8 +295,9 @@ class RaggedCheckpointedSmoother(CheckpointedSmoother):
 
   def run(self, x0, P0, n_ticks, tick_fn, sink, norm_quats=False):
     """x0 [B, DIM], P0 [B, EDIM, EDIM] (host or device).  tick_fn(j, lo, hi) returns tick j of filters lo..hi as the
-    arguments of RaggedScheduler.tick, with filter ids local to the tile: (filter_ids, t, kinds, z_by_kind, R_by_kind) or
-    those and ea_by_kind.  It must return the same tick every time it is asked for j (each tick is filtered twice).
+    arguments of RaggedScheduler.tick, with filter ids local to the tile: (filter_ids, t, kinds, z_by_kind, R_by_kind),
+    those and ea_by_kind, or those and augment (ea_by_kind may be None).  It must return the same tick every time it is
+    asked for j (each tick is filtered twice).
 
     sink(lo, hi, k0 [n], n_rows [n], xs [rows, n, DIM], Ps [rows, n, EDIM, EDIM]) receives, segment by segment (last to
     first), the smoothed rows of filters lo..hi: rows 0 .. n_rows[b] - 1 of filter b are its global rows k0[b] .. (its
